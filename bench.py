@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the cuda_b200 hot path (contract: see DESIGN.md §Measurement).
+"""bench.py — headline benchmark of the cuda_b200 hot path.
 
 A *step* is one full greedy contraction of the closed <psi|psi> network of an L=64,
 bond-dim-512, phys-dim-2 MPS (BASELINE.json configs[1]; 128 tensors -> 127 pairwise
@@ -283,8 +283,18 @@ def workload_config(args, world):
                       % (L_SITES, BOND, PHYS),
           "networks_per_step_per_gpu": max(1, args.networks), "launch_mode": "eager" if args.no_graph else "cuda-graph replay", "compute_dtype": args.dtype, "path_provider": "numpy greedy (opt_einsum stand-in)",
           "parallelism": "replicas x%d (independent MPS samples, no collective)" % world,
-          "l2_policy": "no flush needed: one step reads %d x 128 input tensors = %.1f GB (bf16: 134 MB per network), far beyond the 126 MB L2"
+          "l2_policy": "no flush needed: one step reads %d x 128 input tensors = %.1f GB (bf16: 134 MB per network), far beyond the 50 MB L2"
                        % (max(1, args.networks), max(1, args.networks) * 0.134 * {"bf16": 1, "f32": 2, "f64": 4}[args.dtype])}
+
+
+def dump_outputs(path, arrays):
+  """--dump-outputs: the arrays a caller of the timed path received in its last step, one DIR/<name>.npy each, in
+  float64 when computed in float64 and float32 otherwise.  The inputs are drawn from fixed seeds on the device, so the
+  same arguments give the same inputs in every run."""
+  os.makedirs(path, exist_ok=True)
+  for name, a in arrays.items():
+    a = np.asarray(a)
+    np.save(os.path.join(path, name + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
 
 
 # ------------------------------------------------------------------------------ our arm
@@ -308,6 +318,9 @@ def main():
                   "(no nested sub-records, single BLAS thread setting for the CPU leg)")
   ap.add_argument("--no-strong-scaling", action="store_true", help="N > 1: skip the one-network strong-scaling sub-record")
   ap.add_argument("--no-subrecords", action="store_true", help="skip the by_dtype / configs sub-records of the default line")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy "
+                       "(float32 / float64), so that two builds can be compared output for output")
   args = ap.parse_args()
   quiet_stdout()
   args.warmup = max(args.warmup, 3) if args.impl == "cuda_b200" else max(args.warmup, 1)
@@ -315,6 +328,8 @@ def main():
   world = int(os.environ.get("WORLD_SIZE", "1"))
   local = int(os.environ.get("LOCAL_RANK", "0"))
 
+  if args.dump_outputs and (args.config != "cfg2" or args.impl != "cuda_b200"):
+    ap.error("--dump-outputs covers the timed path of the default line (--config cfg2, --impl cuda_b200)")
   if args.config != "cfg2":
     if rank == 0:
       run_config(args)
@@ -412,6 +427,8 @@ def main():
   launches = (net.launches_per_replay * args.steps) if net is not None else (lib.tnb200_launch_count() - l0)
   ms = e0.elapsed_time(e1)
   result_value = [float(x) for x in np.atleast_1d(res.to_host().astype(np.float64))]
+  if args.dump_outputs:
+    dump_outputs(args.dump_outputs, {"network_values" + ("_rank%d" % rank if world > 1 else ""): res.to_host()})
 
   # ---- latency of ONE network (no sample batching): the same plan compiled for a single MPS sample
   single = None
@@ -525,15 +542,15 @@ def main():
     except Exception:  # pylint: disable=broad-except
       pass
     if args.dtype == "bf16":
-      peak, peak_src = peaks.get("bf16_tflops", 1590.0), ("measured" if peaks else "fallback")
-      peak_note = "bf16 dense (cuBLAS burst), MEASURED_PEAKS.json" if peaks else "fallback 1.59 PF"
+      peak, peak_src = peaks.get("bf16_tflops", 989.0), ("measured" if peaks else "data sheet")
+      peak_note = "bf16 dense (cuBLAS burst), MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet, bf16 dense at 700 W"
     elif args.dtype == "f32":
       peak = measured_peak("tf32")
       peak_src, peak_note = "measured", "tf32 dense: torch.matmul (cuBLAS, allow_tf32) 8192^3, best of 5, measured in this run"
     else:
       peak = measured_peak("f64")
       peak_src, peak_note = "measured", "fp64 dense: torch.matmul (cuBLAS DGEMM) 4096^3, best of 5, measured in this run"
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
+    hbm_peak = peaks.get("hbm_gbs", 3350.0)
     if args.dtype == "bf16" and "bf16_tflops_sustained" in peaks:
       # the dominant kernel is timed inside a long step: the sustained figure is its tensor roof
       peak, peak_note = peaks["bf16_tflops_sustained"], "bf16 dense sustained (cuBLAS back to back), MEASURED_PEAKS.json"
@@ -944,11 +961,11 @@ def run_config(args):
   be = tb.get_backend()
   lib = be.lib
   peaks = _peaks()
-  hbm_peak = peaks.get("hbm_gbs", 6650.0)
+  hbm_peak = peaks.get("hbm_gbs", 3350.0)
   np_dt = {"bf16": np.float32, "f32": np.float32, "f64": np.float64}[args.dtype]
   be_dt = {"bf16": "bfloat16", "f32": np.float32, "f64": np.float64}[args.dtype]
   esize = {"bf16": 2, "f32": 4, "f64": 8}[args.dtype]
-  tensor_peak = peaks.get("bf16_tflops", 1590.0) if args.dtype == "bf16" else measured_peak("tf32" if args.dtype == "f32" else "f64")
+  tensor_peak = peaks.get("bf16_tflops", 989.0) if args.dtype == "bf16" else measured_peak("tf32" if args.dtype == "f32" else "f64")
   fp64_peak = measured_peak("f64")
   peak_source = "MEASURED_PEAKS.json (bf16 burst)" if args.dtype == "bf16" else "cuBLAS %s GEMM measured in this run" % ("tf32" if args.dtype == "f32" else "fp64")
   cand = (16,) if args.sub else (8, 16, 32, 64, None)     # sub-records: one BLAS thread setting (16 was the fastest on this pool's hosts)
@@ -956,7 +973,7 @@ def run_config(args):
   ref_kind = "reference" if tn_ref is not None else "port"
   ref_be = tn_ref.backends.backend_factory.get_backend("numpy") if tn_ref is not None else None
   flushbuf = torch.empty(256 << 20, dtype=torch.uint8, device=be.device)
-  flush = lambda: flushbuf.zero_()                       # 256 MB write > 126 MB L2
+  flush = lambda: flushbuf.zero_()                       # 256 MB write > 50 MB L2
   sampler = ClockSampler(0)
   sampler.start()
   cfg = args.config
@@ -1003,7 +1020,7 @@ def run_config(args):
                               "peak": tensor_peak if t_t >= t_h else hbm_peak, "unit": "TFLOP/s" if t_t >= t_h else "GB/s",
                               "frac": (tf / tensor_peak) if t_t >= t_h else (gbs / hbm_peak), "traffic": None, "kernel": kern,
                               "kernel_tflops": tf, "kernel_gbs": gbs, "peak_source": peak_source,
-                              "note": "single 1.07 GFLOP call on 148 SMs: 32 output tiles of 128x256 -> at most 32 SMs busy; "
+                              "note": "single 1.07 GFLOP call on 132 SMs: 32 output tiles of 128x256 -> at most 32 SMs busy; "
                                       "the batched form of the same shape is the flagship64 record"},
                  "rel_err_vs_fp64": err, "parity_ok": bool(err <= tol),
                  "cpu_baseline": {"value": 1.0 / cpu, "unit": "contractions/s", "cores": cpu_thr, "kind": ref_kind,

@@ -1,4 +1,4 @@
-/* tnb200.h — C ABI of libtnb200.so, the B200-native (sm_100a) dense contraction + split
+/* tnb200.h — C ABI of libtnb200.so, the H100-native (sm_90a) dense contraction + split
  * engine that sits beneath the `cuda_b200` TensorNetwork backend.
  *
  * This is the drop-in boundary of SURVEY.md section 8(b): the reference's plug-in surface is
@@ -64,7 +64,7 @@ typedef struct tnb200_tensor {
 #define TNB200_CONJ_A 0x1
 #define TNB200_CONJ_B 0x2
 /* math mode, bits [4,8): how fp32 / fp64 inputs use the tensor cores */
-#define TNB200_MATH_DEFAULT (0 << 4) /* f64: DMMA fp64; f32: TF32 tcgen05 when large; 16-bit: tcgen05 */
+#define TNB200_MATH_DEFAULT (0 << 4) /* f64: DMMA fp64; f32: TF32 wgmma when large; 16-bit: wgmma */
 #define TNB200_MATH_STRICT (1 << 4)  /* never lower the input precision (f32 -> fp32 FMA path)      */
 #define TNB200_MATH_SIMT (2 << 4)    /* force the generic strided CUDA-core kernel (any dtype)     */
 
@@ -74,7 +74,7 @@ TNB200_API int32_t tnb200_abi_version(void);
 TNB200_API int32_t tnb200_device_info(int32_t* sm_count, int32_t* cc_major, int32_t* cc_minor,
                            int64_t* total_mem);
 /* name of the kernel family the last tnb200_tensordot call on this thread dispatched to
- * ("simt", "dmma_f64", "tcgen05_bf16", ...): used by tests to prove which path ran. */
+ * ("simt", "dmma_f64", "wgmma_bf16", ...): used by tests to prove which path ran. */
 TNB200_API const char* tnb200_last_kernel(void);
 /* number of kernel launches issued by this library since process start (all threads) */
 TNB200_API int64_t tnb200_launch_count(void);

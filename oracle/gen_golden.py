@@ -7,6 +7,7 @@ restatement (tests/test_oracle_golden.py, CPU) and (b) the CUDA path (tests -m g
 """
 import json
 import os
+import sys
 import numpy as np
 from . import ref_shim
 
@@ -358,19 +359,28 @@ def gen_dmrg(tn):
   _save("dmrg", meta, arrays)
 
 
-def main():
+def gen_ref_callers(tn):
+  """What the reference's own callers return on its numpy backend for every case of tests/ref_cases.py: the values
+  tests/test_gpu_reference_callers.py compares the same callers on backend cuda_b200 against."""
+  sys.path.insert(0, os.path.join(os.path.dirname(OUT)))
+  import ref_cases  # pylint: disable=import-outside-toplevel
+  meta, arrays = {}, {}
+  for name, fn, _ in ref_cases.CASES:
+    out = fn(tn, "numpy")
+    meta[name] = len(out)
+    for i, a in enumerate(out):
+      arrays["%s__%d" % (name, i)] = np.asarray(a)
+  _save("ref_callers", meta, arrays)
+
+
+def main(only=()):
   tn = ref_shim.load()
   assert tn.__version__ == "0.4.6"
-  gen_tensordot(tn)
-  gen_ncon(tn)
-  gen_decomp(tn)
-  gen_greedy(tn)
-  gen_split(tn)
-  gen_lanczos(tn)
-  gen_blocksparse(tn)
-  gen_dmrg(tn)
-  gen_symsvd(tn)
+  for gen in (gen_tensordot, gen_ncon, gen_decomp, gen_greedy, gen_split, gen_lanczos, gen_blocksparse, gen_dmrg,
+              gen_symsvd, gen_ref_callers):
+    if not only or gen.__name__[len("gen_"):] in only:
+      gen(tn)
 
 
 if __name__ == "__main__":
-  main()
+  main(sys.argv[1:])

@@ -3,7 +3,7 @@ checks that run the reference's own callers.  Test infrastructure.
 
 The import environment (three third-party stand-ins: h5py, graphviz, opt_einsum — SURVEY.md 8c /
 Appendix A.1) lives in baseline/refenv.py; the package itself is the unmodified copy installed by
-tools/install_ref.sh into baseline/_ref (which travels to the GPU box), else /root/reference.
+build() into oracle/_ref (oracle/install_ref.py), else the upstream checkout it copies from.
 """
 from baseline import refenv
 

@@ -1,4 +1,4 @@
-"""tensornetwork_b200 — B200-native (sm_100a) contraction + split engine behind
+"""tensornetwork_b200 — H100-native (sm_90a) contraction + split engine behind
 google/TensorNetwork's `AbstractBackend` surface, selected with backend="cuda_b200".
 
 Importing this package is cheap: it neither imports torch nor touches CUDA (the reference

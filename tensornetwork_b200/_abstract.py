@@ -1,5 +1,5 @@
 """Mirror of the reference plug-in base class for environments where the `tensornetwork`
-package is not installed (e.g. the GPU box).  Same method names as
+package is not installed (e.g. on a GPU machine without it).  Same method names as
 tensornetwork/backends/abstract_backend.py:22-1046; every operator raises
 NotImplementedError("Backend '<name>' has not implemented <op>.") until a subclass
 provides it (the behaviour tensornetwork/backends/backend_test.py:160ff asserts)."""

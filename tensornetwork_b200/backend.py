@@ -1,4 +1,4 @@
-"""`cuda_b200` — a TensorNetwork backend whose every compute method is a hand-written sm_100a
+"""`cuda_b200` — a TensorNetwork backend whose every compute method is a hand-written sm_90a
 kernel behind the C ABI of libtnb200.so (include/tnb200.h).
 
 Drop-in boundary (SURVEY.md 8b): this class implements the operator surface of
@@ -69,7 +69,7 @@ class CudaB200Backend(_Base):
     dev = _CONFIG["device"]
     if dev is None:
       if not self.torch.cuda.is_available():
-        raise RuntimeError("backend 'cuda_b200' needs a CUDA device (B200, sm_100a); "
+        raise RuntimeError("backend 'cuda_b200' needs a CUDA device (H100, sm_90a); "
                            "there is no CPU fallback")
       dev = self.torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
       self.torch.cuda.set_device(dev)

@@ -1,4 +1,4 @@
-// common.cuh — shared host/device helpers for libtnb200 (sm_100a only).
+// common.cuh — shared host/device helpers for libtnb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -73,7 +73,7 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }

@@ -26,19 +26,19 @@ struct GemmProblem {
   void* C = nullptr; int64_t c_sm = 0, c_sn = 0, c_sb = 0;
   bool conjA = false, conjB = false;
   int math = 0;  // TNB200_MATH_* >> 4
-  bool swapped = false;   // internal: operands exchanged by gemm_tcgen05 (C is written transposed)
+  bool swapped = false;   // internal: operands exchanged by gemm_wgmma (C is written transposed)
 };
 
 // Each returns TNB200_ERR_UNSUPPORTED (without setting an error) when the problem does not
 // meet the kernel's layout/alignment constraints; the planner then repacks or falls back.
-int gemm_tcgen05(const GemmProblem& p, cudaStream_t st);   // bf16 / f16 / f32(tf32)
+int gemm_wgmma(const GemmProblem& p, cudaStream_t st);     // bf16 / f16 / f32(tf32)
 int gemm_dmma_f64(const GemmProblem& p, cudaStream_t st);  // f64 via mma.sync DMMA
-// Chained GEMMs in one persistent launch (gemm_tcgen05.cu): dep_a[i] / dep_b[i] = index of the chain step whose
+// Chained GEMMs in one persistent launch (gemm_wgmma.cu): dep_a[i] / dep_b[i] = index of the chain step whose
 // output is step i's operand A / B (or -1).  create() allocates device tables (call it outside stream capture).
 int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, const int* dep_b, void** handle);
 int gemm_chain_launch(void* handle, cudaStream_t st);
 int gemm_chain_destroy(void* handle);
-// can the TMA/UMMA path address this operand view in place?  (tile-size independent check)
-bool tcgen05_view_ok(int dtype, const OperandView& v, int64_t ext_f, int64_t ext_k, int64_t batch);
+// can the TMA/wgmma path address this operand view in place?  (tile-size independent check)
+bool tma_view_ok(int dtype, const OperandView& v, int64_t ext_f, int64_t ext_k, int64_t batch);
 
 }  // namespace tnb

@@ -1,8 +1,8 @@
 // gemm_dmma.cu — the fp64 path of tnb200_tensordot.
 //
-// tcgen05 has no f64 kind, so double precision runs on the FP64 tensor pipe through
-// mma.sync.aligned.m8n8k4.f64 (DMMA).  B200's FP64 rate is 64 FMA/clk/SM (~40 TFLOP/s), i.e.
-// a 128 x BN x 16 k-block costs >= 2048 cycles of DMMA, which leaves ample room to stage the
+// wgmma has no f64 kind, so double precision runs on the FP64 tensor pipe through
+// mma.sync.aligned.m8n8k4.f64 (DMMA).  H100's FP64 tensor rate is 128 FMA/clk/SM, i.e.
+// a 128 x BN x 16 k-block costs >= 1024 cycles of DMMA, which leaves ample room to stage the
 // operands with plain 8-byte cp.async (LDGSTS): the kernel is FP64-pipe bound by construction.
 // Both operands are arbitrary 2-stride matrices (the tensordot's transposes are folded into
 // the cp.async address computation); shared-memory tiles use the majorness of the global

@@ -1,0 +1,773 @@
+// gemm_wgmma.cu — the tensor-core path of tnb200_tensordot for bf16 / f16 / f32(tf32).
+//
+// One persistent, warp-specialised kernel per launch (H100, sm_90a), 384 threads:
+//   warpgroup 0, warp 0 : TMA producer — cp.async.bulk.tensor (5-D tiled maps built over the *strided
+//                         operand views*, so the tensordot's transpose is performed by the TMA engine),
+//                         SWIZZLE_128B tiles into an S-stage shared-memory ring, mbarrier complete_tx.
+//   warpgroups 1, 2     : consumers — each owns 64 rows of the 128 x BN output tile, issues
+//                         wgmma.mma_async (m64 nBN, K = 32 bytes per instruction) from shared-memory
+//                         descriptors into f32 register accumulators, releases ring slots once the
+//                         MMAs that read them have retired, then stores the tile (converted) to C.
+// 16-bit operands may be K-major (unit stride along the contracted mode) or MN-major (unit stride
+// along the free mode): both are native wgmma layouts (transpose bit).  wgmma reads tf32 operands
+// K-major only, so an MN-major f32 operand is loaded by TMA into a staging slot of the stage and
+// transposed into the K-major layout in shared memory by the consumers — never repacked in HBM.
+// Ragged edges in M, N, K are handled by TMA out-of-bounds zero fill + predicated stores.
+//
+// The chained variant runs a sequence of dependent GEMMs as tiles of the same kernel (see below).
+#include "gemm.cuh"
+#include "wgmma.cuh"
+#include <cuda.h>
+#include <mutex>
+#include <vector>
+
+namespace tnb {
+
+// ------------------------------------------------------------------------ PTX wrappers
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// Bounded wait: a protocol bug traps (visible as a CUDA error) instead of hanging the GPU.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  uint32_t done = 0;
+#pragma unroll 1
+  for (uint32_t it = 0; it < (1u << 28); ++it) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+    if (done) return;
+  }
+  __trap();
+}
+__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// wgmma shared-memory matrix descriptor, 128-byte swizzle.  K-major: rows of 128 bytes, 8-row groups
+// SBO = 1024 B apart (LBO unused).  MN-major: 64-element MN chunks LBO apart, 8-row K groups SBO apart.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+
+struct TcParams {
+  int64_t M, N, K, batch;
+  int BN, num_kb, stages, out_kind;   // out_kind: 0 bf16, 1 f16, 2 f32
+  int64_t tiles_m, tiles_n, num_tiles;
+  int a_mn, b_mn;                     // operand is MN-major
+  // multi-mode operands: extent of the INNER free / contracted mode (0 = the group is one mode).
+  // TMA dims are always (K-major)  [k_in, f_in, f_out, k_out, batch]
+  //                     (MN-major) [f_in, k_in, k_out, f_out, batch]
+  uint32_t a_fe, a_ke, b_fe, b_ke;
+  void* C; int64_t c_sm, c_sb;        // row stride / batch stride of the output tile rows
+  int64_t c_cs;                       // column stride: 1 (normal) or the original row stride (swap-AB: the
+                                      // kernel computes C^T tiles and stores them transposed)
+  int vec_ok;
+};
+
+constexpr int kBM = 128;
+constexpr int kRowBytes = 128;        // one swizzle row = BK elements
+constexpr int kThreads = 384;
+
+// ---------------------------------------------------------------------------------------------
+// Chained GEMMs in ONE persistent launch.
+//
+// A contraction path often contains long runs of dependent GEMMs (the MPS "zipper": E' = A^T (E A) per site).
+// Launched one by one, every step pays the persistent kernel's prologue + drain, and every intermediate makes
+// a round trip through HBM.  Here all steps of such a run are tiles of ONE kernel: the tile sequence is ordered
+// so that a small group of samples is carried through the whole run of steps before the next group starts
+// (intermediates are produced and consumed while still in L2), and inter-step dependencies are tracked per
+// (step, sample) with release/acquire counters in global memory: every consumer warp publishes its part of an
+// output tile with red.release, the TMA producer of a dependent tile spins with ld.acquire + fence.proxy.async
+// before its first load.  Tiles are assigned to CTAs round-robin in sequence order and all CTAs are co-resident
+// (grid <= resident CTAs), so a tile only ever waits for tiles that are earlier in the sequence: no deadlock.
+struct alignas(64) ChainStepDev {
+  CUtensorMap tmA, tmB;
+  TcParams p;
+  int dep_a, dep_b;               // chain step that produces operand a / b (-1: available before the launch)
+  uint32_t need_a, need_b;        // counter value of that step's (sample) entry when it is complete
+  int tiles_per_sample;
+};
+struct ChainSeg { long long tile0; int step, sample0, nsamples, pad; };
+struct ChainParams {
+  const ChainStepDev* steps;
+  const ChainSeg* segs;
+  uint32_t* done;                 // [nsteps][batch] completion counters (zeroed before every launch)
+  long long num_tiles;
+  int nsegs, batch, stages, stage_bytes;
+};
+constexpr int kConsumerWarps = 8;     // consumer warps per CTA: each releases ring slots and publishes its rows of a tile
+
+// Everything one launch needs: a single GEMM (tile params + maps) or a chain.
+struct KernelArgs {
+  CUtensorMap tmA, tmB;
+  TcParams p;
+  ChainParams cp;
+  int stage_bytes;
+};
+
+__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_add_u32(uint32_t* p, uint32_t v) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// bounded spin on a dependency counter (a scheduling bug traps instead of hanging the GPU)
+__device__ __forceinline__ void chain_wait(const uint32_t* ctr, uint32_t need) {
+#pragma unroll 1
+  for (uint32_t it = 0; it < (1u << 24); ++it) {
+    if (ld_acquire_u32(ctr) >= need) return;
+    __nanosleep(64);
+  }
+  __trap();
+}
+
+struct Tile {
+  const TcParams* p;
+  const CUtensorMap *ma, *mb;
+  const ChainStepDev* sd;         // chain step (nullptr for a single GEMM)
+  int bi, mi, ni, step;
+};
+template <bool CHAIN>
+__device__ __forceinline__ void decode_tile(const KernelArgs& a, long long tile, int& cursor, Tile& t) {
+  if (!CHAIN) {
+    uint32_t x = (uint32_t)tile;
+    const uint32_t tn = (uint32_t)a.p.tiles_n, tm = (uint32_t)a.p.tiles_m;
+    t.ni = (int)(x % tn); x /= tn;
+    t.mi = (int)(x % tm);
+    t.bi = (int)(x / tm);
+    t.p = &a.p; t.ma = &a.tmA; t.mb = &a.tmB; t.sd = nullptr; t.step = 0;
+  } else {
+    const ChainParams& cp = a.cp;
+    while (cursor + 1 < cp.nsegs && tile >= cp.segs[cursor + 1].tile0) ++cursor;
+    const ChainSeg sg = cp.segs[cursor];
+    const ChainStepDev* sd = cp.steps + sg.step;
+    uint32_t local = (uint32_t)(tile - sg.tile0);
+    const uint32_t tn = (uint32_t)sd->p.tiles_n, tm = (uint32_t)sd->p.tiles_m;
+    t.ni = (int)(local % tn); local /= tn;
+    t.mi = (int)(local % tm);
+    t.bi = sg.sample0 + (int)(local / tm);
+    t.step = sg.step;
+    t.p = &sd->p; t.ma = &sd->tmA; t.mb = &sd->tmB; t.sd = sd;
+  }
+}
+
+// Transpose the MN-major f32 staging tiles of one stage (TMA layout: chunks of 32 MN elements x 32 K rows,
+// 128-byte rows, 128B swizzle) into the K-major 128B-swizzled rows wgmma reads.  All 256 consumer threads;
+// a warp covers 32 consecutive MN rows of one 16-byte K group: conflict-free reads, 8 rows per store wave.
+__device__ __forceinline__ void transpose_stage_tf32(uint32_t stage, int a_mn, int b_mn, int BN, int ctid) {
+  const uint32_t a_bytes = kBM * kRowBytes, b_bytes = (uint32_t)BN * kRowBytes;
+  const uint32_t staging = stage + a_bytes + b_bytes;
+  const int rows_a = a_mn ? kBM : 0, rows = rows_a + (b_mn ? BN : 0);
+#pragma unroll 1
+  for (int idx = ctid; idx < rows * 8; idx += 256) {
+    const int m = idx & 31, rest = idx >> 5, kc = rest & 7;
+    const int r = (rest >> 3) * 32 + m;                       // row across A rows then B rows
+    const bool is_a = r < rows_a;
+    const int rr = is_a ? r : r - rows_a;
+    const uint32_t src = staging + (is_a ? 0u : a_bytes) + (uint32_t)(rr >> 5) * 4096u;
+    const uint32_t dst = stage + (is_a ? 0u : a_bytes) + (uint32_t)rr * 128u + (uint32_t)((kc ^ (rr & 7)) << 4);
+    uint32_t v[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int k = kc * 4 + i;
+      const uint32_t addr = src + (uint32_t)k * 128u + (uint32_t)((((m >> 2) ^ (k & 7)) << 4) | ((m & 3) << 2));
+      asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v[i]) : "r"(addr) : "memory");
+    }
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma (async proxy) reads
+}
+
+template <int KIND, int BN, int TA, int TB>
+__device__ __forceinline__ void mma_k(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (KIND == 2) {
+    if constexpr (BN == 64) wgmma_n64_tf32(d, a, b, acc);
+    else if constexpr (BN == 128) wgmma_n128_tf32(d, a, b, acc);
+    else wgmma_n256_tf32(d, a, b, acc);
+  } else if constexpr (KIND == 0) {
+    if constexpr (BN == 64) wgmma_n64_bf16<TA, TB>(d, a, b, acc);
+    else if constexpr (BN == 128) wgmma_n128_bf16<TA, TB>(d, a, b, acc);
+    else wgmma_n256_bf16<TA, TB>(d, a, b, acc);
+  } else {
+    if constexpr (BN == 64) wgmma_n64_f16<TA, TB>(d, a, b, acc);
+    else if constexpr (BN == 128) wgmma_n128_f16<TA, TB>(d, a, b, acc);
+    else wgmma_n256_f16<TA, TB>(d, a, b, acc);
+  }
+}
+
+// The k loop of one tile for one consumer warpgroup.  The operand majorness is a template parameter so that
+// the wgmma sequence is straight-line code.  Descriptor fields: a K-major operand advances 32 bytes per MMA,
+// an MN-major one 16 K rows (2 KB); MN chunks of 64 elements are BK rows x 128 B apart.
+template <int KIND, int BN, int TA, int TB>
+__device__ __forceinline__ void mainloop(float* d, uint8_t* smem, int stage_bytes, int S, uint32_t bar_base, int num_kb,
+                                         int a_mn, int b_mn, int wg, int ctid, int lane, int& s, uint32_t& ph) {
+  constexpr int BK = kRowBytes / (KIND == 2 ? 4 : 2);
+  constexpr uint32_t a_lbo = TA ? BK * kRowBytes : 16u, b_lbo = TB ? BK * kRowBytes : 16u;
+  constexpr uint32_t a_kstep = TA ? 16u * kRowBytes : 32u, b_kstep = TB ? 16u * kRowBytes : 32u;
+  int prev = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(bar_base + 8u * s, ph);
+    const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+    if (KIND == 2 && (a_mn || b_mn)) {
+      transpose_stage_tf32(sa, a_mn, b_mn, BN, ctid);
+      consumers_sync();
+    }
+    const uint32_t sa_wg = sa + (uint32_t)wg * 64u * kRowBytes;   // 64 rows (K-major) = one 64-element chunk (MN-major)
+    const uint32_t sb = sa + kBM * kRowBytes;
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      mma_k<KIND, BN, TA, TB>(d, gmma_desc(sa_wg + k * a_kstep, a_lbo, 1024u), gmma_desc(sb + k * b_kstep, b_lbo, 1024u),
+                              (kb > 0 || k > 0) ? 1u : 0u);
+    wg_commit();
+    if (prev >= 0) {
+      wg_wait<1>();                                            // the MMAs of the previous stage have retired
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_base + 8u * (S + prev));
+    }
+    prev = s;
+    if (++s == S) { s = 0; ph ^= 1; }
+  }
+  wg_wait<0>();
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar_base + 8u * (S + prev));
+}
+
+__device__ __forceinline__ void store_one(const TcParams& p, int64_t off, float v) {
+  if (p.out_kind == 2) ((float*)p.C)[off] = v;
+  else if (p.out_kind == 0) ((__nv_bfloat16*)p.C)[off] = __float2bfloat16_rn(v);
+  else ((__half*)p.C)[off] = __float2half_rn(v);
+}
+__device__ __forceinline__ void store_pair(const TcParams& p, int64_t off, float v0, float v1) {
+  if (p.out_kind == 2) *(float2*)((float*)p.C + off) = make_float2(v0, v1);
+  else if (p.out_kind == 0) *(__nv_bfloat162*)((__nv_bfloat16*)p.C + off) = __floats2bfloat162_rn(v0, v1);
+  else *(__half2*)((__half*)p.C + off) = __floats2half2_rn(v0, v1);
+}
+
+template <int KIND, int BN, bool CHAIN>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
+  constexpr int ES = KIND == 2 ? 4 : 2;          // operand element bytes
+  constexpr int BK = kRowBytes / ES;             // 64 (16-bit) or 32 (tf32) elements per k-block
+  constexpr int CHUNK = kRowBytes / ES;          // MN elements per 128-byte row of an MN-major tile
+  constexpr int A_BYTES = kBM * kRowBytes;       // 16 KB per stage
+  constexpr int B_BYTES = BN * kRowBytes;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const int STAGE_BYTES = args.stage_bytes;
+  const int S = CHAIN ? args.cp.stages : args.p.stages;
+  const long long num_tiles = CHAIN ? args.cp.num_tiles : args.p.num_tiles;
+  uint64_t* bars = (uint64_t*)(smem + (size_t)S * STAGE_BYTES);
+  const uint32_t bar_base = smem_u32(bars);
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };       // bars: full[S], empty[S]
+  auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    if (!CHAIN) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&args.tmA) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&args.tmB) : "memory");
+    }
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  const long long first = blockIdx.x, step = gridDim.x;
+
+  if (warp == 0) {
+    // ===================================================== TMA producer (whole warp)
+    // lane l owns "load slot" l of a stage: one 128-byte-wide box of A (slots 0..nA-1) or of B (nA..nA+nB-1),
+    // so the boxes of a stage are issued in parallel; inside the k loop a lane only advances its contracted-mode
+    // coordinates incrementally.
+    int s = 0; uint32_t ph = 0;
+    int cursor = 0;
+    for (long long tile = first; tile < num_tiles; tile += step) {
+      Tile t;
+      decode_tile<CHAIN>(args, tile, cursor, t);
+      const TcParams& p = *t.p;
+      const int a_mn = p.a_mn, b_mn = p.b_mn;
+      const int nA = a_mn ? kBM / CHUNK : 1;
+      const int nB = b_mn ? BN / CHUNK : 1;
+      const bool mine = lane < nA + nB;
+      const bool is_a = lane < nA;
+      const int c = is_a ? lane : lane - nA;                       // chunk index inside the operand tile
+      const bool mn = is_a ? (a_mn != 0) : (b_mn != 0);
+      const uint32_t fe = is_a ? p.a_fe : p.b_fe, ke = is_a ? p.a_ke : p.b_ke;
+      const CUtensorMap* map = is_a ? t.ma : t.mb;
+      uint32_t dst_off = (is_a ? 0u : (uint32_t)A_BYTES) + (mn ? (uint32_t)c * (BK * kRowBytes) : 0u);
+      if (KIND == 2 && mn) dst_off += A_BYTES + B_BYTES;          // f32 MN-major: staging slot, transposed by the consumers
+      const int f = is_a ? t.mi * kBM + (mn ? c * CHUNK : 0) : t.ni * BN + (mn ? c * CHUNK : 0);
+      const int f_in = fe ? (int)((uint32_t)f % fe) : f, f_out = fe ? (int)((uint32_t)f / fe) : 0;
+      const int num_kb = p.num_kb;
+      if (CHAIN) {
+        // operands produced by earlier steps of this launch: wait until every tile of (that step, this sample) is out
+        if (lane == 0) {
+          const ChainStepDev* sd = t.sd;
+          if (sd->dep_a >= 0) chain_wait(args.cp.done + (size_t)sd->dep_a * args.cp.batch + t.bi, sd->need_a);
+          if (sd->dep_b >= 0) chain_wait(args.cp.done + (size_t)sd->dep_b * args.cp.batch + t.bi, sd->need_b);
+        }
+        __syncwarp();
+        asm volatile("fence.proxy.async;" ::: "memory");     // generic-proxy writes (other SMs' epilogues) -> our TMA reads
+      }
+      int k_in = 0, k_out = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(empty_bar(s), ph ^ 1);                          // slot free (every lane observes it)
+        const uint32_t full = full_bar(s);
+        if (lane == 0) mbar_expect_tx(full, (uint32_t)(A_BYTES + B_BYTES));
+        __syncwarp();
+        if (mine) {
+          const uint32_t dst = smem_u32(smem + (size_t)s * STAGE_BYTES) + dst_off;
+          if (!mn) tma_load_5d(dst, map, full, k_in, f_in, f_out, k_out, t.bi);
+          else     tma_load_5d(dst, map, full, f_in, k_in, k_out, f_out, t.bi);
+        }
+        k_in += BK;
+        if (ke && (uint32_t)k_in >= ke) { k_in = 0; ++k_out; }
+        if (++s == S) { s = 0; ph ^= 1; }
+      }
+    }
+  } else if (warp >= 4) {
+    // ===================================================== consumers: MMA + epilogue
+    const int ctid = threadIdx.x - 128;                           // 0..255
+    const int wg = ctid >> 7;                                     // rows 64 wg .. 64 wg + 63 of the tile
+    const int wt = ctid & 127;
+    int s = 0; uint32_t ph = 0;
+    int cursor = 0;
+    float d[BN / 2];
+    for (long long tile = first; tile < num_tiles; tile += step) {
+      Tile t;
+      decode_tile<CHAIN>(args, tile, cursor, t);
+      const TcParams& p = *t.p;
+      const int a_mn = p.a_mn, b_mn = p.b_mn, num_kb = p.num_kb;
+      if constexpr (KIND == 2) {
+        mainloop<KIND, BN, 0, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+      } else {
+        if (a_mn && b_mn) mainloop<KIND, BN, 1, 1>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        else if (a_mn) mainloop<KIND, BN, 1, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        else if (b_mn) mainloop<KIND, BN, 0, 1>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        else mainloop<KIND, BN, 0, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+      }
+      // ---- epilogue straight from the accumulator registers
+      const int r0 = (wt >> 5) * 16 + (lane >> 2);
+      const int64_t row0 = (int64_t)t.mi * kBM + wg * 64 + r0;
+      const int64_t n0 = (int64_t)t.ni * BN + 2 * (lane & 3);
+      const int64_t cb = (int64_t)t.bi * p.c_sb;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = row0 + 8 * h;
+        if (row < p.M) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int64_t col = n0 + 8 * j;
+            const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+            if (p.c_cs == 1) {
+              const int64_t off = cb + row * p.c_sm + col;
+              if (p.vec_ok && col + 1 < p.N) store_pair(p, off, v0, v1);
+              else {
+                if (col < p.N) store_one(p, off, v0);
+                if (col + 1 < p.N) store_one(p, off + 1, v1);
+              }
+            } else {
+              const int64_t off = cb + row * p.c_sm + col * p.c_cs;
+              if (col < p.N) store_one(p, off, v0);
+              if (col + 1 < p.N) store_one(p, off + p.c_cs, v1);
+            }
+          }
+        }
+      }
+      if (CHAIN) {
+        __threadfence();
+        __syncwarp();
+        if (lane == 0) red_release_add_u32(args.cp.done + (size_t)t.step * args.cp.batch + t.bi, 1u);
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------- host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static EncodeTiledFn get_encode() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, []() {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = (EncodeTiledFn)p;
+  });
+  return fn;
+}
+
+static int es_of(int dt) { return dt == TNB200_F32 ? 4 : 2; }
+static int kind_of(int dt) { return dt == TNB200_BF16 ? 0 : (dt == TNB200_F16 ? 1 : 2); }
+
+// Which operand majorness can serve this view?  0: K-major, 1: MN-major, -1: neither (needs a repack).
+// Conditions (es = element bytes, R = 128/es elements per swizzle row):
+//   * unit stride on the innermost contracted mode (K-major) or innermost free mode (MN-major);
+//   * every other stride and the base pointer 16-byte aligned; rank <= 5 (<= 2 modes per group);
+//   * two contracted modes: inner extent % R == 0 (a k-block never straddles the mode boundary);
+//   * two free modes: MN-major: inner extent % R == 0;  K-major: inner extent % 256 == 0, or a
+//     power of two <= 64 (so every tile size 64/128/256 either divides it or is a multiple of it).
+static int view_major(int dtype, const OperandView& v, int64_t ext_f, int64_t ext_k, int64_t batch) {
+  if (dtype != TNB200_F32 && dtype != TNB200_F16 && dtype != TNB200_BF16) return -1;
+  const int es = es_of(dtype);
+  const int64_t R = kRowBytes / es;
+  if (((uintptr_t)v.ptr) & 15) return -1;
+  if (v.nF > 2 || v.nK > 2) return -1;
+  if (ext_f >= (1LL << 31) || ext_k >= (1LL << 31) || batch >= (1LL << 31)) return -1;
+  auto ok16 = [&](int64_t s) { return s > 0 && (s * es) % 16 == 0 && s * es < (1LL << 40); };
+  if (batch > 1 && !ok16(v.sb)) return -1;
+  if (v.nK == 2 && v.ke[1] % R != 0) return -1;
+  const bool k_unit = ext_k == 1 || v.nK == 0 || v.ks[v.nK - 1] == 1;
+  const bool f_unit = ext_f == 1 || v.nF == 0 || v.fs[v.nF - 1] == 1;
+  if (k_unit) {  // K-major candidate: all free strides + outer K stride must be 16B multiples
+    bool ok = true;
+    for (int i = 0; i < v.nF; ++i) ok = ok && (v.fe[i] == 1 || ok16(v.fs[i]));
+    if (v.nK == 2) ok = ok && ok16(v.ks[0]);
+    if (v.nF == 2) { int64_t e = v.fe[1]; ok = ok && (e % 256 == 0 || (e <= 64 && (e & (e - 1)) == 0)); }
+    if (ok) return 0;
+  }
+  if (f_unit) {
+    bool ok = true;
+    for (int i = 0; i < v.nK; ++i) ok = ok && (v.ke[i] == 1 || ok16(v.ks[i]));
+    if (v.nF == 2) ok = ok && ok16(v.fs[0]) && (v.fe[1] % R == 0);
+    if (ok) return 1;
+  }
+  return -1;
+}
+
+bool tma_view_ok(int dtype, const OperandView& v, int64_t ext_f, int64_t ext_k, int64_t batch) {
+  return view_major(dtype, v, ext_f, ext_k, batch) >= 0;
+}
+
+// Build the rank-5 tensor map of one operand for tiles of `tile` free rows.
+static int encode_operand(CUtensorMap* map, int dtype, const OperandView& v, int64_t ext_f, int64_t ext_k, int64_t batch,
+                          int tile, bool& mn_major, uint32_t& fe_in, uint32_t& ke_in) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return TNB200_ERR_UNSUPPORTED;
+  const int major = view_major(dtype, v, ext_f, ext_k, batch);
+  if (major < 0) return TNB200_ERR_UNSUPPORTED;
+  mn_major = major == 1;
+  const int es = es_of(dtype);
+  const int R = kRowBytes / es;
+  CUtensorMapDataType cdt = dtype == TNB200_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                            : (dtype == TNB200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+  // (extent, stride) of inner / outer mode of each group; missing modes are extent 1
+  int64_t f_in_e = v.nF ? v.fe[v.nF - 1] : 1, f_in_s = v.nF ? v.fs[v.nF - 1] : 0;
+  int64_t f_out_e = v.nF == 2 ? v.fe[0] : 1, f_out_s = v.nF == 2 ? v.fs[0] : 0;
+  int64_t k_in_e = v.nK ? v.ke[v.nK - 1] : 1, k_in_s = v.nK ? v.ks[v.nK - 1] : 0;
+  int64_t k_out_e = v.nK == 2 ? v.ke[0] : 1, k_out_s = v.nK == 2 ? v.ks[0] : 0;
+  fe_in = v.nF == 2 ? (uint32_t)f_in_e : 0u;
+  ke_in = v.nK == 2 ? (uint32_t)k_in_e : 0u;
+  int64_t de[5], ds[5];   // extents, element strides (ds[0] is the unit-stride dim)
+  cuuint32_t box[5] = {1, 1, 1, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
+  if (!mn_major) {
+    de[0] = k_in_e; ds[0] = 1;
+    de[1] = f_in_e; ds[1] = f_in_s; de[2] = f_out_e; ds[2] = f_out_s;
+    de[3] = k_out_e; ds[3] = k_out_s; de[4] = batch; ds[4] = v.sb;
+    box[0] = R;
+    if (v.nF == 2 && f_in_e < tile) {
+      if (tile % f_in_e) return TNB200_ERR_UNSUPPORTED;
+      box[1] = (cuuint32_t)f_in_e; box[2] = (cuuint32_t)(tile / f_in_e);
+    } else {
+      if (v.nF == 2 && f_in_e % tile) return TNB200_ERR_UNSUPPORTED;
+      box[1] = tile;
+    }
+  } else {
+    de[0] = f_in_e; ds[0] = 1;
+    de[1] = k_in_e; ds[1] = k_in_s; de[2] = k_out_e; ds[2] = k_out_s;
+    de[3] = f_out_e; ds[3] = f_out_s; de[4] = batch; ds[4] = v.sb;
+    box[0] = R; box[1] = R;   // R elements of the free mode (128 B) x BK = R contracted rows
+  }
+  cuuint64_t dims[5], strides[4];
+  int64_t natural = 16;   // bytes: a packed stride for extent-1 (never addressed) dims
+  for (int d = 0; d < 5; ++d) {
+    dims[d] = (cuuint64_t)(de[d] < 1 ? 1 : de[d]);
+    int64_t bytes = es;
+    if (d > 0) {
+      bytes = ds[d] * es;
+      if (de[d] <= 1) bytes = (natural + 15) / 16 * 16;
+      else if (bytes <= 0 || bytes % 16) return TNB200_ERR_UNSUPPORTED;
+      strides[d - 1] = (cuuint64_t)bytes;
+    }
+    if ((int64_t)dims[d] * bytes > natural) natural = (int64_t)dims[d] * bytes;
+  }
+  CUresult r = enc(map, cdt, 5, const_cast<void*>(v.ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return TNB200_ERR_UNSUPPORTED;
+  return 0;
+}
+
+// bytes of one ring stage: A and B tiles, plus the staging slots of f32 MN-major operands
+static int stage_bytes_of(int dtype, int BN, bool a_mn, bool b_mn) {
+  const int kmajor = kBM * kRowBytes + BN * kRowBytes;
+  return (dtype == TNB200_F32 && (a_mn || b_mn)) ? 2 * kmajor : kmajor;
+}
+constexpr int kRingBudget = 200 * 1024;
+
+struct TcPrep {
+  TcParams p;
+  CUtensorMap tmA, tmB;
+  int stage_bytes;
+};
+
+// Tile selection and tensor maps of one GEMM.  chain_mode: the problem is one step of a chained launch, whose
+// steps share one kernel instance: always 128 x 128 tiles.
+static int tc_prepare(const GemmProblem& g, bool chain_mode, TcPrep& o) {
+  TcParams& p = o.p;
+  const int es = es_of(g.dtype);
+  const int sms = num_sms();
+  const int64_t tiles_m = (g.M + kBM - 1) / kBM;
+  int BN = 64;   // multiples of 64 so that an MN-major B tile is a whole number of 128-byte chunks
+  if (chain_mode) {
+    BN = 128;
+  } else if (!g.swapped) {
+    const int cands[3] = {256, 128, 64};
+    for (int i = 0; i < 3; ++i) {
+      int bn = cands[i];
+      if (bn > 64 && bn / 2 >= g.N) continue;          // tile mostly empty
+      int64_t tiles = tiles_m * ((g.N + bn - 1) / bn) * g.batch;
+      if (tiles >= sms || bn == 64) { BN = bn; break; }
+    }
+  }
+  p.M = g.M; p.N = g.N; p.K = g.K; p.batch = g.batch;
+  p.BN = BN;
+  const int bk = kRowBytes / es;
+  p.num_kb = (int)((g.K + bk - 1) / bk);
+  p.tiles_m = tiles_m;
+  p.tiles_n = (g.N + BN - 1) / BN;
+  p.num_tiles = p.tiles_m * p.tiles_n * g.batch;
+  p.out_kind = g.dtype == TNB200_BF16 ? 0 : (g.dtype == TNB200_F16 ? 1 : 2);
+  p.C = g.C; p.c_sm = g.c_sm; p.c_sb = g.c_sb; p.c_cs = g.swapped ? g.c_sn : 1;
+  if (g.swapped && p.c_cs == 1) p.c_cs = 2;   // degenerate (M == 1): force the transposed-store path; stride unused
+  p.vec_ok = !g.swapped && (((uintptr_t)g.C) % 16 == 0) && ((g.c_sm * es) % 16 == 0) && ((g.c_sb * es) % 16 == 0);
+  bool a_mn = false, b_mn = false;
+  int rc = encode_operand(&o.tmA, g.dtype, g.A, g.M, g.K, g.batch, kBM, a_mn, p.a_fe, p.a_ke);
+  if (rc) return rc;
+  rc = encode_operand(&o.tmB, g.dtype, g.B, g.N, g.K, g.batch, BN, b_mn, p.b_fe, p.b_ke);
+  if (rc) return rc;
+  p.a_mn = a_mn; p.b_mn = b_mn;
+  o.stage_bytes = stage_bytes_of(g.dtype, BN, a_mn, b_mn);
+  int stages = kRingBudget / o.stage_bytes;
+  if (stages > 8) stages = 8;
+  if (stages > p.num_kb + 1 && p.num_tiles <= sms) stages = p.num_kb + 1 > 2 ? p.num_kb + 1 : 2;
+  p.stages = stages;
+  return 0;
+}
+
+typedef void (*KernelFn)(KernelArgs);
+static KernelFn kernel_of(int kind, int BN, bool chain) {
+#define TNB_K(K) (chain ? (KernelFn)gemm_wgmma_kernel<K, 128, true>                                   \
+                        : (BN == 64 ? (KernelFn)gemm_wgmma_kernel<K, 64, false>                      \
+                                    : (BN == 128 ? (KernelFn)gemm_wgmma_kernel<K, 128, false>        \
+                                                 : (KernelFn)gemm_wgmma_kernel<K, 256, false>)))
+  return kind == 0 ? TNB_K(0) : (kind == 1 ? TNB_K(1) : TNB_K(2));
+#undef TNB_K
+}
+static size_t smem_of(int stages, int stage_bytes) { return (size_t)stages * stage_bytes + 2 * stages * 8 + 1024; }
+static int raise_smem(KernelFn fn) {
+  cudaError_t e = cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  if (e != cudaSuccess) { set_error("wgmma: cannot raise dynamic smem: %s", cudaGetErrorString(e)); return TNB200_ERR_CUDA; }
+  return 0;
+}
+
+int gemm_wgmma(const GemmProblem& g, cudaStream_t st) {
+  if (g.dtype != TNB200_F32 && g.dtype != TNB200_F16 && g.dtype != TNB200_BF16) return TNB200_ERR_UNSUPPORTED;
+  if (g.conjA || g.conjB) return TNB200_ERR_UNSUPPORTED;
+  if (!g.swapped && g.c_sn != 1 && g.N > 1) return TNB200_ERR_UNSUPPORTED;
+  if (g.swapped && g.c_sm != 1 && g.M > 1) return TNB200_ERR_UNSUPPORTED;
+  if (g.M >= (1LL << 31) || g.N >= (1LL << 31) || g.K >= (1LL << 31)) return TNB200_ERR_UNSUPPORTED;
+  if (!tma_view_ok(g.dtype, g.A, g.M, g.K, g.batch) || !tma_view_ok(g.dtype, g.B, g.N, g.K, g.batch))
+    return TNB200_ERR_UNSUPPORTED;
+  // swap-AB: a tiny M under a large N would waste the 128-row tile; compute C^T = B^T A^T instead
+  // (the big free dimension rides the 128 tile rows, the tiny one a 64-column tile) and let the
+  // epilogue store the tile transposed.
+  if (g.M <= 64 && g.N >= 128 && !g.swapped) {
+    GemmProblem t = g;
+    t.swapped = true;
+    t.M = g.N; t.N = g.M; t.A = g.B; t.B = g.A;
+    t.c_sm = g.c_sn; t.c_sn = g.c_sm;          // row stride of C^T = column stride of C (1)
+    return gemm_wgmma(t, st);
+  }
+  KernelArgs args;
+  memset(&args, 0, sizeof(args));
+  {
+    TcPrep prep;
+    int rc = tc_prepare(g, false, prep);
+    if (rc) return rc;
+    args.tmA = prep.tmA; args.tmB = prep.tmB; args.p = prep.p; args.stage_bytes = prep.stage_bytes;
+  }
+  const int kind = kind_of(g.dtype);
+  KernelFn fn = kernel_of(kind, args.p.BN, false);
+  static bool attr_set[3][3] = {};
+  const int bi = args.p.BN == 64 ? 0 : (args.p.BN == 128 ? 1 : 2);
+  if (!attr_set[kind][bi]) {
+    int rc = raise_smem(fn);
+    if (rc) return rc;
+    attr_set[kind][bi] = true;
+  }
+  const int64_t sms = num_sms();
+  const int64_t grid = args.p.num_tiles < sms ? args.p.num_tiles : sms;
+  fn<<<(unsigned)grid, kThreads, smem_of(args.p.stages, args.stage_bytes), st>>>(args);
+  TNB_LAUNCH_CHECK();
+  count_launch();
+  set_kernel_name(kind == 0 ? "wgmma_bf16" : (kind == 1 ? "wgmma_f16" : "wgmma_tf32"));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------- chain: host side
+struct ChainHandle {
+  ChainStepDev* d_steps = nullptr;
+  ChainSeg* d_segs = nullptr;
+  uint32_t* d_done = nullptr;
+  KernelArgs args;
+  int kind = 0, nsteps = 0;
+  size_t smem = 0, done_bytes = 0;
+  unsigned grid = 0;
+};
+
+int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, const int* dep_b, void** handle) {
+  *handle = nullptr;
+  if (nsteps < 1) return TNB200_ERR_INVALID;
+  {
+    static int disabled = -1;
+    if (disabled < 0) { const char* e = getenv("TNB200_NO_CHAIN"); disabled = (e && e[0] == '1') ? 1 : 0; }
+    if (disabled) return TNB200_ERR_UNSUPPORTED;
+  }
+  const int dtype = probs[0].dtype;
+  const int64_t batch = probs[0].batch;
+  std::vector<ChainStepDev> steps(nsteps);
+  int max_stage = 0;
+  for (int i = 0; i < nsteps; ++i) {
+    const GemmProblem& g = probs[i];
+    if (g.dtype != dtype || g.batch != batch || g.conjA || g.conjB || g.swapped) return TNB200_ERR_UNSUPPORTED;
+    if (g.dtype != TNB200_F32 && g.dtype != TNB200_F16 && g.dtype != TNB200_BF16) return TNB200_ERR_UNSUPPORTED;
+    if (g.c_sn != 1 || g.M >= (1LL << 31) || g.N >= (1LL << 31) || g.K >= (1LL << 31)) return TNB200_ERR_UNSUPPORTED;
+    if (dep_a[i] >= i || dep_b[i] >= i) return TNB200_ERR_INVALID;
+    TcPrep prep;
+    int rc = tc_prepare(g, true, prep);
+    if (rc) return rc;
+    ChainStepDev& sd = steps[i];
+    memset(&sd, 0, sizeof(sd));
+    sd.tmA = prep.tmA; sd.tmB = prep.tmB; sd.p = prep.p;
+    sd.dep_a = dep_a[i]; sd.dep_b = dep_b[i];
+    sd.tiles_per_sample = (int)(prep.p.tiles_m * prep.p.tiles_n);
+    if (prep.stage_bytes > max_stage) max_stage = prep.stage_bytes;
+  }
+  for (int i = 0; i < nsteps; ++i) {
+    if (steps[i].dep_a >= 0) steps[i].need_a = kConsumerWarps * (uint32_t)steps[steps[i].dep_a].tiles_per_sample;
+    if (steps[i].dep_b >= 0) steps[i].need_b = kConsumerWarps * (uint32_t)steps[steps[i].dep_b].tiles_per_sample;
+  }
+  const int kind = kind_of(dtype);
+  KernelFn fn = kernel_of(kind, 128, true);
+  {
+    static bool attr_set[3] = {};
+    if (!attr_set[kind]) {
+      int rc = raise_smem(fn);
+      if (rc) return rc;
+      attr_set[kind] = true;
+    }
+  }
+  int stages = kRingBudget / max_stage;
+  if (stages > 8) stages = 8;
+  if (stages < 2) return TNB200_ERR_UNSUPPORTED;
+  const size_t smem = smem_of(stages, max_stage);
+  // every CTA of the launch must be resident (tiles wait on earlier tiles): ask the runtime how many fit
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)fn, kThreads, smem) != cudaSuccess) { cudaGetLastError(); per_sm = 0; }
+  const int ctas = per_sm * num_sms();
+  if (ctas < 1) return TNB200_ERR_UNSUPPORTED;
+  // ---- tile sequence.  The batch is cut into rounds of G samples and every round is carried through ALL steps
+  // before the next one starts, so a step's results are consumed soon after they are produced; a round must be
+  // wide enough that a dependent tile is >= 2 full waves of tiles behind its producers.
+  auto env_int = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
+  int min_tps = steps[0].tiles_per_sample;
+  for (int i = 1; i < nsteps; ++i) if (steps[i].tiles_per_sample < min_tps) min_tps = steps[i].tiles_per_sample;
+  if (batch * min_tps < ctas && !env_int("TNB200_CHAIN_FORCE", 0))
+    return TNB200_ERR_UNSUPPORTED;      // too few tiles per step to hide the producer->consumer latency: launch step by step
+  int G = env_int("TNB200_CHAIN_G", (2 * ctas + min_tps - 1) / min_tps);
+  if (G < 1) G = 1;
+  std::vector<ChainSeg> segs;
+  long long tile0 = 0;
+  for (int64_t r0 = 0; r0 < batch; r0 += G) {
+    const int64_t r1 = r0 + G < batch ? r0 + G : batch;
+    for (int i = 0; i < nsteps; ++i) {
+      ChainSeg sg;
+      sg.tile0 = tile0; sg.step = i; sg.sample0 = (int)r0; sg.nsamples = (int)(r1 - r0); sg.pad = 0;
+      segs.push_back(sg);
+      tile0 += (long long)(r1 - r0) * steps[i].tiles_per_sample;
+    }
+  }
+  ChainHandle* h = new ChainHandle();
+  h->kind = kind;
+  h->nsteps = nsteps;
+  h->done_bytes = sizeof(uint32_t) * (size_t)nsteps * (size_t)batch;
+  cudaError_t e = cudaMalloc(&h->d_steps, sizeof(ChainStepDev) * steps.size());
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_segs, sizeof(ChainSeg) * segs.size());
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_done, h->done_bytes);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_steps, steps.data(), sizeof(ChainStepDev) * steps.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_segs, segs.data(), sizeof(ChainSeg) * segs.size(), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    set_error("chain: device table allocation failed: %s", cudaGetErrorString(e));
+    cudaFree(h->d_steps); cudaFree(h->d_segs); cudaFree(h->d_done);
+    delete h;
+    return TNB200_ERR_CUDA;
+  }
+  memset(&h->args, 0, sizeof(h->args));
+  ChainParams& cp = h->args.cp;
+  cp.steps = h->d_steps; cp.segs = h->d_segs; cp.done = h->d_done;
+  cp.num_tiles = tile0; cp.nsegs = (int)segs.size(); cp.batch = (int)batch;
+  cp.stages = stages; cp.stage_bytes = max_stage;
+  h->args.stage_bytes = max_stage;
+  h->smem = smem;
+  h->grid = (unsigned)(tile0 < ctas ? tile0 : ctas);
+  *handle = h;
+  return 0;
+}
+
+int gemm_chain_launch(void* handle, cudaStream_t st) {
+  ChainHandle* h = (ChainHandle*)handle;
+  if (!h) return TNB200_ERR_INVALID;
+  TNB_CHECK_CUDA(cudaMemsetAsync(h->d_done, 0, h->done_bytes, st));
+  kernel_of(h->kind, 128, true)<<<h->grid, kThreads, h->smem, st>>>(h->args);
+  TNB_LAUNCH_CHECK();
+  count_launch();
+  set_kernel_name(h->kind == 2 ? "wgmma_chain_tf32" : "wgmma_chain_16");
+  return 0;
+}
+
+int gemm_chain_destroy(void* handle) {
+  ChainHandle* h = (ChainHandle*)handle;
+  if (!h) return 0;
+  cudaFree(h->d_steps); cudaFree(h->d_segs); cudaFree(h->d_done);
+  delete h;
+  return 0;
+}
+
+}  // namespace tnb

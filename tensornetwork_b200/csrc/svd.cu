@@ -809,9 +809,8 @@ __global__ void svd_trunc_kernel(const T* __restrict__ s, int64_t n, int64_t str
 using namespace tnb;
 
 // Block width: 16.  The 32-wide variant (half the rounds per sweep, i.e. half the HBM traffic of the gram / update
-// kernels) is kept for real dtypes behind TNB200_SVD_SB=32, but it is SLOWER on B200 — measured 2048^2: 0.57 s vs
-// 0.37 s, 4096^2: 2.20 s vs 2.06 s, same sweep counts — because the 64 x 64 Gram eigenproblem (63 dependent Jacobi
-// steps per inner sweep in one CTA) then dominates every round.
+// kernels) is kept for real dtypes behind TNB200_SVD_SB=32.  It is not the default: the 64 x 64 Gram eigenproblem
+// (63 dependent Jacobi steps per inner sweep in one CTA) then dominates every round.
 static int svd_dispatch(bool cplx, const tnb200_tensor_t* a, const tnb200_tensor_t* u, const tnb200_tensor_t* s, const tnb200_tensor_t* vh,
                         int32_t* info_dev, cudaStream_t st) {
   if (cplx) return svd_real<zd, 16>(a, u, s, vh, info_dev, st);

@@ -4,7 +4,7 @@
 // Replaces NumPyBackend.tensordot (backends/numpy/numpy_backend.py:35-54) and the batched
 // matmul of ncon's _batch_cont (ncon_interface.py:280-354).  np.tensordot materialises
 // transposed copies of both operands and calls BLAS; here the operand permutation is folded
-// into the kernel's address computation (SIMT path) or into TMA tensor maps (tcgen05 path).
+// into the kernel's address computation (SIMT path) or into TMA tensor maps (wgmma path).
 #include "gemm.cuh"
 #include <algorithm>
 #include <vector>
@@ -347,7 +347,7 @@ int build_modes(const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200
   return 0;
 }
 
-// Lower a contraction to a GEMM whose operands are BOTH addressable in place by the TMA / tcgen05 path
+// Lower a contraction to a GEMM whose operands are BOTH addressable in place by the TMA / wgmma path
 // (no repack, no skinny / thin special case).  Used by the chained-GEMM planner (gemm_chain.cu).
 int plan_inplace_gemm(const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200_tensor_t* c, int32_t naxes,
                       const int32_t* axes_a, const int32_t* axes_b, int32_t nbatch, const int32_t* batch_a,
@@ -381,7 +381,7 @@ int plan_inplace_gemm(const tnb200_tensor_t* a, const tnb200_tensor_t* b, const 
     va.nK = vb.nK = ko.n;
     for (int i = 0; i < ko.n; ++i) { va.ke[i] = vb.ke[i] = ko.ext[i]; va.ks[i] = ko.s0[i]; vb.ks[i] = ko.s1[i]; }
     va.sb = gB.n ? gB.s0[0] : 0; vb.sb = gB.n ? gB.s1[0] : 0;
-    if (tcgen05_view_ok(dt, va, M, K, Bt) && tcgen05_view_ok(dt, vb, N, K, Bt)) {
+    if (tma_view_ok(dt, va, M, K, Bt) && tma_view_ok(dt, vb, N, K, Bt)) {
       g.A = va; g.B = vb;
       return 0;
     }
@@ -455,7 +455,7 @@ extern "C" int32_t tnb200_tensordot(const tnb200_tensor_t* a, const tnb200_tenso
       };
       auto view_ok = [&](const OperandView& v, int64_t ef) -> bool {
         if (dt == TNB200_F64) return v.simple();
-        return tcgen05_view_ok(dt, v, ef, K, Bt);
+        return tma_view_ok(dt, v, ef, K, Bt);
       };
       int best = -1, best_score = -1; bool bestA = false, bestB = false;
       OperandView va, vb;
@@ -496,7 +496,7 @@ extern "C" int32_t tnb200_tensordot(const tnb200_tensor_t* a, const tnb200_tenso
             for (int i = ip.nK - 1; i >= 0; --i) { pk.ke[i] = ip.ke[i]; pk.ks[i] = st_; st_ *= ip.ke[i]; }
           }
           g.A = va; g.B = vb;
-          rc = (dt == TNB200_F64) ? gemm_dmma_f64(g, st) : gemm_tcgen05(g, st);
+          rc = (dt == TNB200_F64) ? gemm_dmma_f64(g, st) : gemm_wgmma(g, st);
           if (rc == TNB200_ERR_UNSUPPORTED && (bestA || bestB) && !(packA && packB)) {
             // in-place addressing was rejected at encode time (tile-size dependent): repack everything
             if (!packA) {
@@ -511,7 +511,7 @@ extern "C" int32_t tnb200_tensordot(const tnb200_tensor_t* a, const tnb200_tenso
               rc = pack_operand(dt, b->data, gB, 1, nB, ko, 1, &packB, &kp, st);
               vb = OperandView(); vb.ptr = packB; vb.nF = 1; vb.fe[0] = N; vb.fs[0] = kp; vb.nK = 1; vb.ke[0] = K; vb.ks[0] = 1; vb.sb = N * kp;
             } else if (packB) { vb.nK = 1; vb.ke[0] = K; vb.ks[0] = 1; }
-            if (rc == 0) { g.A = va; g.B = vb; rc = (dt == TNB200_F64) ? gemm_dmma_f64(g, st) : gemm_tcgen05(g, st); }
+            if (rc == 0) { g.A = va; g.B = vb; rc = (dt == TNB200_F64) ? gemm_dmma_f64(g, st) : gemm_wgmma(g, st); }
           }
         }
         if (packA) ws_free(packA, st);
@@ -545,7 +545,7 @@ extern "C" int32_t tnb200_chain_create(int32_t nsteps, const tnb200_chain_step_t
   // tile-shape eligibility is per step: report the first step the chained kernel cannot take
   for (int i = 0; i < nsteps; ++i) {
     const GemmProblem& g = probs[i];
-    if (g.M < 256 || g.N < 128 || g.batch != probs[0].batch || g.dtype != probs[0].dtype) {
+    if (g.M < 128 || g.N < 128 || g.batch != probs[0].batch || g.dtype != probs[0].dtype) {
       if (first_unsupported) *first_unsupported = i;
       return TNB200_ERR_UNSUPPORTED;
     }

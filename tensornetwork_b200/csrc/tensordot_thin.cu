@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(256) thin_mma_kernel(const __grid_constant__ T
 
 // ------------------------------------------------------------------------------------------ warp MMA, fp32 as TF32
 // Same scheme with mma.sync.m16n8k8 (tf32 inputs = the fp32 bit patterns, fp32 accumulate — the precision class of the
-// tcgen05 kind::tf32 path these shapes would otherwise take).  K = 8*KT8 in {16, 32, 64}; P <= 16*PT.
+// wgmma tf32 path these shapes would otherwise take).  K = 8*KT8 in {16, 32, 64}; P <= 16*PT.
 __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])

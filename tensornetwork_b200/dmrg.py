@@ -4,7 +4,7 @@ With the `tensornetwork` package installed, the reference's own `FiniteDMRG.run_
 (matrixproductstates/dmrg.py:445-559) runs unchanged on `backend="cuda_b200"`
 (tests/test_refhost.py).  This module restates that driver — same ncon networks, same sweep
 order, same Lanczos / SVD calls — without depending on the reference package, so cfg 5 can be
-run and timed on a GPU box where the reference is absent:
+run and timed on a GPU machine where the reference is absent:
 
   two_site_matvec  <-> dmrg.py:95-100       add_left/right_layer <-> dmrg.py:102-112
   position (QR/RQ) <-> base_mps.py:139-226   _optimize_2s_local   <-> dmrg.py:251-343

@@ -1,9 +1,10 @@
 """Row N1: the reference's own callers, UNMODIFIED, on backend="cuda_b200" with the real kernels.
 
-The reference package is the pip-installed copy under baseline/_ref (tools/install_ref.sh), imported
-through baseline/refenv.py.  Every case of tests/ref_cases.py is run with backend="numpy" (the
-reference's own numpy backend) and backend="cuda_b200" in the same process, on the same seeded
-inputs, and compared (fp64: <= 1e-10 of the result scale; integers exact)."""
+The reference package is the unmodified copy build() puts under oracle/_ref, imported through
+baseline/refenv.py.  Every case of tests/ref_cases.py is run with backend="cuda_b200" on seeded inputs and
+compared with what the same callers returned on the reference's own numpy backend for those inputs
+(tests/golden/ref_callers.npz, written by oracle/gen_golden.py; fp64: <= 1e-10 of the result scale;
+integers exact)."""
 import numpy as np
 import pytest
 import ref_cases
@@ -23,12 +24,13 @@ def _backend(tn):
 
 
 @pytest.mark.parametrize("name,fn,tol", ref_cases.CASES, ids=[c[0] for c in ref_cases.CASES])
-def test_reference_caller(tn, name, fn, tol):
+def test_reference_caller(tn, golden, name, fn, tol):
   be = _backend(tn)
   n0 = be.lib.tnb200_launch_count()
   got = fn(tn, "cuda_b200")
   launches = be.lib.tnb200_launch_count() - n0
-  ref = fn(tn, "numpy")
+  meta, z = golden("ref_callers")
+  ref = [z["%s__%d" % (name, i)] for i in range(meta[name])]
   ref_cases.compare(name, got, ref, tol)
   assert launches > 0, "no libtnb200 kernel ran for " + name
 
@@ -64,7 +66,7 @@ def test_reference_error_conventions(tn):
 
 def test_reference_greedy_mps_norm_D64_float32_and_complex(tn):
   """A larger <psi|psi> through contractors.greedy (path_contractors.py:87-90): the per-pair loop
-  reaches the tcgen05 / DMMA / thin kernels rather than only the SIMT fallback.  float32 is checked
+  reaches the wgmma / DMMA / thin kernels rather than only the SIMT fallback.  float32 is checked
   twice: strict (fp32 FMA, 1e-4 after 23 chained contractions) and the tensor-core TF32 mode, whose
   2^-11 operand rounding accumulates over the chain (stated tolerance 2e-2)."""
   from tensornetwork_b200 import _lib as L

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05/TMA tensor-core path (bf16 / f16 / tf32) against float64 numpy on
+"""GPU parity of the wgmma/TMA tensor-core path (bf16 / f16 / tf32) against float64 numpy on
 identically rounded inputs.  Tolerances: bf16 4e-3 (output rounding 2^-9), f16 1e-3, tf32 1e-3
 (10-bit mantissa inputs, fp32 accumulate), all relative Frobenius."""
 import numpy as np
@@ -28,7 +28,7 @@ def test_two_site_all_majors(dtype, axes):
   B, b = _mk(be, rng, (256, 2, 256), dtype)
   out = be.tensordot(A, B, axes)
   kern = be.lib.tnb200_last_kernel().decode()
-  assert kern.startswith("tcgen05"), kern
+  assert kern.startswith("wgmma"), kern
   ref = np.tensordot(a, b, axes)
   e = rel_err(out.to_host(), ref)
   assert e < TOLS[dtype], "%s %s via %s: %.3e" % (dtype, axes, kern, e)
@@ -60,7 +60,7 @@ def test_batched(dtype):
   A, a = _mk(be, rng, (6, 256, 128), dtype)
   B, b = _mk(be, rng, (6, 128, 192), dtype)
   out = be.matmul(A, B)
-  assert be.lib.tnb200_last_kernel().decode().startswith("tcgen05")
+  assert be.lib.tnb200_last_kernel().decode().startswith("wgmma")
   assert rel_err(out.to_host(), np.matmul(a, b)) < TOLS[dtype]
 
 
@@ -102,7 +102,7 @@ def test_multimode_operands_are_fused_not_repacked(dtype):
   l0 = _launches(be)
   out = be.tensordot(A, Tt, ([0, 1], [2, 0]))
   assert _launches(be) - l0 == 1, "repacked: %d launches" % (_launches(be) - l0)
-  assert be.lib.tnb200_last_kernel().decode().startswith("tcgen05")
+  assert be.lib.tnb200_last_kernel().decode().startswith("wgmma")
   assert rel_err(out.to_host(), np.tensordot(a, t, ([0, 1], [2, 0]))) < TOLS[dtype]
   # free group = two modes around the contracted physical leg (MN-major, inner extent % 64 == 0)
   X, x = _mk(be, rng, (256, 4, 128), dtype)
@@ -137,7 +137,7 @@ def test_swap_ab_tiny_m(dtype):
     B, b = _mk(be, rng, (k, n), dtype)
     out = be.tensordot(A, B, 1)
     kern = be.lib.tnb200_last_kernel().decode()     # short K + tiny M streams through the CUDA-core kernel
-    assert kern.startswith("tcgen05") or kern == "skinny_outer", (m, k, n, kern)
+    assert kern.startswith("wgmma") or kern == "skinny_outer", (m, k, n, kern)
     assert rel_err(out.to_host(), a @ b) < TOLS[dtype], (m, k, n)
     Bt, bt = _mk(be, rng, (n, k), dtype)          # K-major big operand
     out = be.tensordot(A, be.transpose(Bt), 1)
@@ -234,5 +234,5 @@ def test_thin_fp32_strict_mode_stays_fp32():
     kern = be.lib.tnb200_last_kernel().decode()
   finally:
     be.math_mode = old
-  assert "tf32" not in kern and not kern.startswith("tcgen05"), kern
+  assert "tf32" not in kern and not kern.startswith("wgmma"), kern
   assert rel_err(out.to_host(), np.einsum("bpk,bkl->bpl", s, x)) < 2e-5

@@ -22,7 +22,7 @@ def test_golden_tensordot():
     assert out.dtype == z["out%d" % i].dtype
     kern = be.lib.tnb200_last_kernel().decode()
     # float32 on the tensor cores is TF32 (10-bit mantissa): stated tolerance 2e-3
-    tol = TOL["tf32"] if kern.startswith("tcgen05") else None
+    tol = TOL["tf32"] if kern.startswith("wgmma") else None
     assert_close(out, z["out%d" % i], tol=tol, what="golden tensordot case %d via %s" % (i, kern))
 
 
@@ -53,7 +53,7 @@ def test_oracle_random(dtype, case):
   out = be.tensordot(be.convert_to_tensor(a), be.convert_to_tensor(b), axes)
   assert out.shape == ref.shape
   kern = be.lib.tnb200_last_kernel().decode()
-  tol = TOL["tf32"] if (dtype == "float32" and kern.startswith("tcgen05")) else None   # fp32 on tensor cores = TF32
+  tol = TOL["tf32"] if (dtype == "float32" and kern.startswith("wgmma")) else None   # fp32 on tensor cores = TF32
   assert_close(out, ref.astype(dtype) if dtype.startswith("int") else ref, dtype=dtype, tol=tol)
 
 

@@ -10,7 +10,7 @@ from oracle import ref_shim
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = [pytest.mark.refhost,
-              pytest.mark.skipif(not ref_shim.available(), reason="/root/reference not present (GPU box)")]
+              pytest.mark.skipif(not ref_shim.available(), reason="upstream TensorNetwork checkout not present")]
 
 
 def _run(*extra):

@@ -1,4 +1,4 @@
-"""Kernel-level throughput probe (GPU box only): times N back-to-back launches of one tensordot
+"""Kernel-level throughput probe (needs a GPU): times N back-to-back launches of one tensordot
 shape with CUDA events, so that the host round trip is amortised.  Prints one JSON line per case."""
 import json
 import sys

@@ -1,4 +1,4 @@
-"""QR timing probe (GPU box only): tnb200_qr on m x n fp64, CUDA events.  python tools/qr_bench.py 2048x1024 4096x4096"""
+"""QR timing probe (needs a GPU): tnb200_qr on m x n fp64, CUDA events.  python tools/qr_bench.py 2048x1024 4096x4096"""
 import json
 import os
 import sys

@@ -1,4 +1,4 @@
-"""SVD timing probe (GPU box only): tnb200_svd on n x n fp64 matrices, CUDA events, sweeps from the info words.
+"""SVD timing probe (needs a GPU): tnb200_svd on n x n fp64 matrices, CUDA events, sweeps from the info words.
 python tools/svd_bench.py 1024 2048 4096 [--f32]"""
 import json
 import os
