@@ -14,7 +14,8 @@
 // transposed into the K-major layout in shared memory by the consumers — never repacked in HBM.
 // Ragged edges in M, N, K are handled by TMA out-of-bounds zero fill + predicated stores.
 //
-// The chained variant runs a sequence of dependent GEMMs as tiles of the same kernel (see below).
+// The chained variant runs a sequence of dependent GEMMs as tiles of the same kernel (see below); its
+// consumers hand the tile to warp 1, which stores it with TMA while they start the next tile.
 #include "gemm.cuh"
 #include "wgmma.cuh"
 #include <cuda.h>
@@ -54,6 +55,13 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
 }
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -98,15 +106,23 @@ constexpr int kThreads = 384;
 // a round trip through HBM.  Here all steps of such a run are tiles of ONE kernel: the tile sequence is ordered
 // so that a small group of samples is carried through the whole run of steps before the next group starts
 // (intermediates are produced and consumed while still in L2), and inter-step dependencies are tracked per
-// (step, sample) with release/acquire counters in global memory: every consumer warp publishes its part of an
-// output tile with red.release, the TMA producer of a dependent tile spins with ld.acquire + fence.proxy.async
-// before its first load.  Tiles are assigned to CTAs round-robin in sequence order and all CTAs are co-resident
-// (grid <= resident CTAs), so a tile only ever waits for tiles that are earlier in the sequence: no deadlock.
+// (step, sample) with release/acquire counters in global memory: once the TMA stores of an output tile have
+// completed, the CTA's store warp publishes the tile with red.release, the TMA producer of a dependent tile spins
+// with ld.acquire + fence.proxy.async before its first load.  Tiles are assigned to CTAs round-robin in sequence
+// order and all CTAs are co-resident (grid <= resident CTAs), so a tile only ever waits for tiles that are earlier
+// in the sequence: no deadlock.
+//
+// The chain's epilogue overlaps the next tile's k loop: the consumers convert the accumulators into a shared-memory
+// staging buffer (128-byte swizzled 64-row x 128-byte boxes: conflict-free stores) and go on to the next tile; warp
+// 1 writes the buffer out with TMA stores through a per-step tensor map of C, frees it once the TMA engine has
+// read it, and publishes the tile once the stores are complete.  16-bit chains run 128 x 256 tiles (3 ring stages
+// of 48 KB + 64 KB staging), tf32 chains 128 x 128 (their MN-major transpose slot doubles a stage, so their 32 KB
+// tile half is staged in two 16 KB passes to keep 3 stages of 64 KB).
 struct alignas(64) ChainStepDev {
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmC;
   TcParams p;
   int dep_a, dep_b;               // chain step that produces operand a / b (-1: available before the launch)
-  uint32_t need_a, need_b;        // counter value of that step's (sample) entry when it is complete
+  uint32_t need_a, need_b;        // counter value of that step's (sample) entry when it is complete: its tiles
   int tiles_per_sample;
 };
 struct ChainSeg { long long tile0; int step, sample0, nsamples, pad; };
@@ -117,7 +133,11 @@ struct ChainParams {
   long long num_tiles;
   int nsegs, batch, stages, stage_bytes;
 };
-constexpr int kConsumerWarps = 8;     // consumer warps per CTA: each releases ring slots and publishes its rows of a tile
+constexpr int kConsumerWarps = 8;     // consumer warps per CTA: each releases ring slots
+// Chain epilogue staging, per consumer warpgroup (64 rows x 512 bytes of output = four 8 KB boxes).
+constexpr int kChainBN16 = 256, kChainBN32 = 128;
+constexpr int kBoxBytes = 64 * 128;
+constexpr int chain_stage_half(int kind) { return kind == 2 ? 2 * kBoxBytes : 4 * kBoxBytes; }
 
 // Everything one launch needs: a single GEMM (tile params + maps) or a chain.
 struct KernelArgs {
@@ -135,6 +155,23 @@ __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
 __device__ __forceinline__ void red_release_add_u32(uint32_t* p, uint32_t v) {
   asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+#ifdef TNB200_CHAIN_PHASES
+// Diagnostic build only (tools/chain_phases.py; never part of the library): per CTA, nanoseconds of %globaltimer
+// spent in each phase of the chained kernel, accumulated over launches.  Each slot has a single writer thread.
+constexpr int kPhases = 6;        // producer chain_wait, consumer full-barrier wait, k loop, epilogue, CTA lifetime, tiles
+constexpr int kPhaseCtas = 1024;
+__device__ unsigned long long g_chain_phase[kPhaseCtas * kPhases];
+__device__ __forceinline__ unsigned long long phase_clock() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
+  return t;
+}
+#define TNB_PHASE(...) __VA_ARGS__
+#define TNB_PHASE_ADD(slot, v) (g_chain_phase[blockIdx.x * kPhases + (slot)] += (v))
+#else
+#define TNB_PHASE(...)
+#endif
+
 // bounded spin on a dependency counter (a scheduling bug traps instead of hanging the GPU)
 __device__ __forceinline__ void chain_wait(const uint32_t* ctr, uint32_t need) {
 #pragma unroll 1
@@ -230,7 +267,9 @@ __device__ __forceinline__ void mainloop(float* d, uint8_t* smem, int stage_byte
   constexpr uint32_t a_kstep = TA ? 16u * kRowBytes : 32u, b_kstep = TB ? 16u * kRowBytes : 32u;
   int prev = -1;
   for (int kb = 0; kb < num_kb; ++kb) {
+    TNB_PHASE(const unsigned long long tw = phase_clock();)
     mbar_wait(bar_base + 8u * s, ph);
+    TNB_PHASE(if (ctid == 0) TNB_PHASE_ADD(1, phase_clock() - tw);)
     const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
     if (KIND == 2 && (a_mn || b_mn)) {
       transpose_stage_tf32(sa, a_mn, b_mn, BN, ctid);
@@ -281,18 +320,26 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
   const int STAGE_BYTES = args.stage_bytes;
   const int S = CHAIN ? args.cp.stages : args.p.stages;
   const long long num_tiles = CHAIN ? args.cp.num_tiles : args.p.num_tiles;
-  uint64_t* bars = (uint64_t*)(smem + (size_t)S * STAGE_BYTES);
+  // chain: the epilogue staging buffer (one half per consumer warpgroup) follows the ring
+  constexpr int STAGE_HALF = chain_stage_half(KIND);
+  const uint32_t staging = smem_u32(smem + (size_t)S * STAGE_BYTES);
+  uint64_t* bars = (uint64_t*)(smem + (size_t)S * STAGE_BYTES + (CHAIN ? 2 * STAGE_HALF : 0));
   const uint32_t bar_base = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };       // bars: full[S], empty[S]
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };       // bars: full[S], empty[S], staged[2], freed[2]
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
+  auto staged_bar = [&](int wg) { return bar_base + 8u * (2 * S + wg); };
+  auto freed_bar = [&](int wg) { return bar_base + 8u * (2 * S + 2 + wg); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  TNB_PHASE(const unsigned long long t_start = phase_clock();)
   if (threadIdx.x == 0) {
     if (!CHAIN) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&args.tmA) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&args.tmB) : "memory");
     }
     for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
+    if (CHAIN)
+      for (int wg = 0; wg < 2; ++wg) { mbar_init(staged_bar(wg), 4); mbar_init(freed_bar(wg), 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -326,9 +373,11 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
       if (CHAIN) {
         // operands produced by earlier steps of this launch: wait until every tile of (that step, this sample) is out
         if (lane == 0) {
+          TNB_PHASE(const unsigned long long tw = phase_clock();)
           const ChainStepDev* sd = t.sd;
           if (sd->dep_a >= 0) chain_wait(args.cp.done + (size_t)sd->dep_a * args.cp.batch + t.bi, sd->need_a);
           if (sd->dep_b >= 0) chain_wait(args.cp.done + (size_t)sd->dep_b * args.cp.batch + t.bi, sd->need_b);
+          TNB_PHASE(TNB_PHASE_ADD(0, phase_clock() - tw);)
         }
         __syncwarp();
         asm volatile("fence.proxy.async;" ::: "memory");     // generic-proxy writes (other SMs' epilogues) -> our TMA reads
@@ -355,6 +404,7 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
     const int wg = ctid >> 7;                                     // rows 64 wg .. 64 wg + 63 of the tile
     const int wt = ctid & 127;
     int s = 0; uint32_t ph = 0;
+    uint32_t eph = 0;                                             // chain: staging-buffer phase
     int cursor = 0;
     float d[BN / 2];
     for (long long tile = first; tile < num_tiles; tile += step) {
@@ -362,6 +412,7 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
       decode_tile<CHAIN>(args, tile, cursor, t);
       const TcParams& p = *t.p;
       const int a_mn = p.a_mn, b_mn = p.b_mn, num_kb = p.num_kb;
+      TNB_PHASE(const unsigned long long tk = phase_clock();)
       if constexpr (KIND == 2) {
         mainloop<KIND, BN, 0, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
       } else {
@@ -370,8 +421,44 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
         else if (b_mn) mainloop<KIND, BN, 0, 1>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
         else mainloop<KIND, BN, 0, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
       }
-      // ---- epilogue straight from the accumulator registers
+      TNB_PHASE(const unsigned long long te = phase_clock(); if (ctid == 0) TNB_PHASE_ADD(2, te - tk);)
       const int r0 = (wt >> 5) * 16 + (lane >> 2);
+      if constexpr (CHAIN) {
+        // ---- epilogue into the staging buffer; warp 1 stores it.  Accumulator d[4j + 2h + e] is row r0 + 8h,
+        // column 8j + 2(lane & 3) + e; a box holds 128 bytes of 64 rows, its 16-byte chunk c of row r at c ^ (r & 7).
+        constexpr int J_PER_PASS = BN / 8 * STAGE_HALF / (4 * kBoxBytes);
+        const uint32_t half = staging + (uint32_t)wg * STAGE_HALF;
+#pragma unroll
+        for (int pass = 0; pass < 4 * kBoxBytes / STAGE_HALF; ++pass) {
+          mbar_wait(freed_bar(wg), eph ^ 1);                       // the store warp has read the previous contents
+#pragma unroll
+          for (int jj = 0; jj < J_PER_PASS; ++jj) {
+            const int j = pass * J_PER_PASS + jj;
+            const uint32_t colb = (uint32_t)(8 * j + 2 * (lane & 3)) * ES - (uint32_t)pass * STAGE_HALF / 64;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t r = (uint32_t)(r0 + 8 * h);
+              const uint32_t addr = half + (colb >> 7) * kBoxBytes + r * 128u + ((((colb >> 4) & 7) ^ (r & 7)) << 4) + (colb & 15);
+              const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+              if constexpr (KIND == 2) {
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
+              } else {
+                uint32_t u;
+                if constexpr (KIND == 0) { __nv_bfloat162 x = __floats2bfloat162_rn(v0, v1); u = *(uint32_t*)&x; }
+                else { __half2 x = __floats2half2_rn(v0, v1); u = *(uint32_t*)&x; }
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(u) : "memory");
+              }
+            }
+          }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> TMA (async proxy) reads
+          __syncwarp();
+          if (lane == 0) mbar_arrive(staged_bar(wg));
+          eph ^= 1;
+        }
+        TNB_PHASE(if (ctid == 0) { TNB_PHASE_ADD(3, phase_clock() - te); TNB_PHASE_ADD(5, 1); })
+        continue;
+      }
+      // ---- epilogue straight from the accumulator registers
       const int64_t row0 = (int64_t)t.mi * kBM + wg * 64 + r0;
       const int64_t n0 = (int64_t)t.ni * BN + 2 * (lane & 3);
       const int64_t cb = (int64_t)t.bi * p.c_sb;
@@ -398,11 +485,39 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
           }
         }
       }
-      if (CHAIN) {
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) red_release_add_u32(args.cp.done + (size_t)t.step * args.cp.batch + t.bi, 1u);
+    }
+    TNB_PHASE(if (ctid == 0) TNB_PHASE_ADD(4, phase_clock() - t_start);)
+  } else if (CHAIN && warp == 1 && lane == 0) {
+    // ===================================================== chain: store warp
+    int cursor = 0;
+    uint32_t sph = 0;
+    for (long long tile = first; tile < num_tiles; tile += step) {
+      Tile t;
+      decode_tile<CHAIN>(args, tile, cursor, t);
+      const CUtensorMap* mc = &t.sd->tmC;
+#pragma unroll 1
+      for (int pass = 0; pass < 4 * kBoxBytes / STAGE_HALF; ++pass) {
+#pragma unroll 1
+        for (int wg = 0; wg < 2; ++wg) {
+          mbar_wait(staged_bar(wg), sph);
+          for (int b = 0; b < STAGE_HALF / kBoxBytes; ++b) {
+            const int box = pass * (STAGE_HALF / kBoxBytes) + b;
+            tma_store_3d(mc, staging + (uint32_t)(wg * STAGE_HALF + b * kBoxBytes), t.ni * BN + box * (128 / ES),
+                         t.mi * kBM + wg * 64, t.bi);
+          }
+          bulk_commit();
+          bulk_wait_read_all();
+          mbar_arrive(freed_bar(wg));
+        }
+        sph ^= 1;
       }
+      // Publish the tile.  wait_group (without .read) returns once the bulk stores are complete, i.e. their writes
+      // to global memory have been performed.  Those writes belong to the async proxy; fence.proxy.async orders them
+      // with this thread's generic-proxy accesses, so the red.release that follows publishes them at gpu scope.  A
+      // dependent producer pairs it with ld.acquire and its own fence.proxy.async before its TMA (async-proxy) loads.
+      bulk_wait_all();
+      asm volatile("fence.proxy.async.global;" ::: "memory");
+      red_release_add_u32(args.cp.done + (size_t)t.step * args.cp.batch + t.bi, 1u);
     }
   }
 }
@@ -524,6 +639,24 @@ static int encode_operand(CUtensorMap* map, int dtype, const OperandView& v, int
   return 0;
 }
 
+// Tensor map of a chain step's output C = [batch][M rows at c_sm][N contiguous] for the TMA-store epilogue:
+// boxes of 64 rows x 128 bytes in the 128-byte swizzle the consumers stage them in.  TMA clips ragged edges.
+static int encode_output(CUtensorMap* map, const GemmProblem& g) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return TNB200_ERR_UNSUPPORTED;
+  const int64_t es = es_of(g.dtype);
+  if (((uintptr_t)g.C) & 15 || g.c_sm <= 0 || (g.c_sm * es) % 16) return TNB200_ERR_UNSUPPORTED;
+  if (g.batch > 1 && (g.c_sb <= 0 || (g.c_sb * es) % 16)) return TNB200_ERR_UNSUPPORTED;
+  const CUtensorMapDataType cdt = g.dtype == TNB200_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                  : (g.dtype == TNB200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+  cuuint64_t dims[3] = {(cuuint64_t)g.N, (cuuint64_t)g.M, (cuuint64_t)g.batch};
+  cuuint64_t strides[2] = {(cuuint64_t)(g.c_sm * es), (cuuint64_t)((g.batch > 1 ? g.c_sb : g.M * g.c_sm) * es)};
+  cuuint32_t box[3] = {(cuuint32_t)(kRowBytes / es), 64, 1}, estr[3] = {1, 1, 1};
+  CUresult r = enc(map, cdt, 3, g.C, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : TNB200_ERR_UNSUPPORTED;
+}
+
 // bytes of one ring stage: A and B tiles, plus the staging slots of f32 MN-major operands
 static int stage_bytes_of(int dtype, int BN, bool a_mn, bool b_mn) {
   const int kmajor = kBM * kRowBytes + BN * kRowBytes;
@@ -538,7 +671,7 @@ struct TcPrep {
 };
 
 // Tile selection and tensor maps of one GEMM.  chain_mode: the problem is one step of a chained launch, whose
-// steps share one kernel instance: always 128 x 128 tiles.
+// steps share one kernel instance: 128 x 256 tiles (16-bit) or 128 x 128 (tf32).
 static int tc_prepare(const GemmProblem& g, bool chain_mode, TcPrep& o) {
   TcParams& p = o.p;
   const int es = es_of(g.dtype);
@@ -546,7 +679,7 @@ static int tc_prepare(const GemmProblem& g, bool chain_mode, TcPrep& o) {
   const int64_t tiles_m = (g.M + kBM - 1) / kBM;
   int BN = 64;   // multiples of 64 so that an MN-major B tile is a whole number of 128-byte chunks
   if (chain_mode) {
-    BN = 128;
+    BN = g.dtype == TNB200_F32 ? kChainBN32 : kChainBN16;
   } else if (!g.swapped) {
     const int cands[3] = {256, 128, 64};
     for (int i = 0; i < 3; ++i) {
@@ -583,7 +716,7 @@ static int tc_prepare(const GemmProblem& g, bool chain_mode, TcPrep& o) {
 
 typedef void (*KernelFn)(KernelArgs);
 static KernelFn kernel_of(int kind, int BN, bool chain) {
-#define TNB_K(K) (chain ? (KernelFn)gemm_wgmma_kernel<K, 128, true>                                   \
+#define TNB_K(K) (chain ? (KernelFn)gemm_wgmma_kernel<K, (K == 2 ? kChainBN32 : kChainBN16), true>        \
                         : (BN == 64 ? (KernelFn)gemm_wgmma_kernel<K, 64, false>                      \
                                     : (BN == 128 ? (KernelFn)gemm_wgmma_kernel<K, 128, false>        \
                                                  : (KernelFn)gemm_wgmma_kernel<K, 256, false>)))
@@ -664,6 +797,7 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
   const int64_t batch = probs[0].batch;
   std::vector<ChainStepDev> steps(nsteps);
   int max_stage = 0;
+  int64_t sample_bytes = 0;       // largest per-sample footprint of one step: both operands and the result
   for (int i = 0; i < nsteps; ++i) {
     const GemmProblem& g = probs[i];
     if (g.dtype != dtype || g.batch != batch || g.conjA || g.conjB || g.swapped) return TNB200_ERR_UNSUPPORTED;
@@ -675,17 +809,21 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
     if (rc) return rc;
     ChainStepDev& sd = steps[i];
     memset(&sd, 0, sizeof(sd));
+    rc = encode_output(&sd.tmC, g);
+    if (rc) return rc;
     sd.tmA = prep.tmA; sd.tmB = prep.tmB; sd.p = prep.p;
     sd.dep_a = dep_a[i]; sd.dep_b = dep_b[i];
     sd.tiles_per_sample = (int)(prep.p.tiles_m * prep.p.tiles_n);
     if (prep.stage_bytes > max_stage) max_stage = prep.stage_bytes;
+    const int64_t b = (g.M * g.K + g.N * g.K + g.M * g.N) * es_of(dtype);
+    if (b > sample_bytes) sample_bytes = b;
   }
   for (int i = 0; i < nsteps; ++i) {
-    if (steps[i].dep_a >= 0) steps[i].need_a = kConsumerWarps * (uint32_t)steps[steps[i].dep_a].tiles_per_sample;
-    if (steps[i].dep_b >= 0) steps[i].need_b = kConsumerWarps * (uint32_t)steps[steps[i].dep_b].tiles_per_sample;
+    if (steps[i].dep_a >= 0) steps[i].need_a = (uint32_t)steps[steps[i].dep_a].tiles_per_sample;
+    if (steps[i].dep_b >= 0) steps[i].need_b = (uint32_t)steps[steps[i].dep_b].tiles_per_sample;
   }
   const int kind = kind_of(dtype);
-  KernelFn fn = kernel_of(kind, 128, true);
+  KernelFn fn = kernel_of(kind, 0, true);
   {
     static bool attr_set[3] = {};
     if (!attr_set[kind]) {
@@ -694,29 +832,44 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
       attr_set[kind] = true;
     }
   }
-  int stages = kRingBudget / max_stage;
+  // the ring gets what the 227 KB of shared memory leave beside the epilogue staging and the barriers
+  const int staging = 2 * chain_stage_half(kind);
+  int stages = (227 * 1024 - 1024 - staging - 256) / max_stage;
   if (stages > 8) stages = 8;
   if (stages < 2) return TNB200_ERR_UNSUPPORTED;
-  const size_t smem = smem_of(stages, max_stage);
+  const size_t smem = smem_of(stages, max_stage) + staging + 4 * 8;
   // every CTA of the launch must be resident (tiles wait on earlier tiles): ask the runtime how many fit
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)fn, kThreads, smem) != cudaSuccess) { cudaGetLastError(); per_sm = 0; }
   const int ctas = per_sm * num_sms();
   if (ctas < 1) return TNB200_ERR_UNSUPPORTED;
-  // ---- tile sequence.  The batch is cut into rounds of G samples and every round is carried through ALL steps
-  // before the next one starts, so a step's results are consumed soon after they are produced; a round must be
-  // wide enough that a dependent tile is >= 2 full waves of tiles behind its producers.
+  // ---- tile sequence.  The batch is cut into rounds of about G samples and every round is carried through ALL
+  // steps before the next one starts, so a step's results are consumed soon after they are produced.  A round
+  // must be wide enough that a dependent tile is at least one full wave of tiles behind its producers, and should
+  // be as wide as the L2 allows: the operands and results of one step of the round then stay in L2 for the next.
   auto env_int = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
   int min_tps = steps[0].tiles_per_sample;
   for (int i = 1; i < nsteps; ++i) if (steps[i].tiles_per_sample < min_tps) min_tps = steps[i].tiles_per_sample;
   if (batch * min_tps < ctas && !env_int("TNB200_CHAIN_FORCE", 0))
     return TNB200_ERR_UNSUPPORTED;      // too few tiles per step to hide the producer->consumer latency: launch step by step
-  int G = env_int("TNB200_CHAIN_G", (2 * ctas + min_tps - 1) / min_tps);
+  int l2 = 0;
+  {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) != cudaSuccess) {
+      cudaGetLastError();
+      l2 = 0;
+    }
+  }
+  const int g_wave = (ctas + min_tps - 1) / min_tps;
+  const int g_l2 = (int)(l2 / sample_bytes);
+  int G = env_int("TNB200_CHAIN_G", g_wave > g_l2 ? g_wave : g_l2);
   if (G < 1) G = 1;
+  // balanced rounds: ceil(batch / G) of them, sizes differing by at most one sample
+  const int64_t rounds = (batch + G - 1) / G;
   std::vector<ChainSeg> segs;
   long long tile0 = 0;
-  for (int64_t r0 = 0; r0 < batch; r0 += G) {
-    const int64_t r1 = r0 + G < batch ? r0 + G : batch;
+  for (int64_t r = 0; r < rounds; ++r) {
+    const int64_t r0 = batch * r / rounds, r1 = batch * (r + 1) / rounds;
     for (int i = 0; i < nsteps; ++i) {
       ChainSeg sg;
       sg.tile0 = tile0; sg.step = i; sg.sample0 = (int)r0; sg.nsamples = (int)(r1 - r0); sg.pad = 0;
@@ -755,7 +908,7 @@ int gemm_chain_launch(void* handle, cudaStream_t st) {
   ChainHandle* h = (ChainHandle*)handle;
   if (!h) return TNB200_ERR_INVALID;
   TNB_CHECK_CUDA(cudaMemsetAsync(h->d_done, 0, h->done_bytes, st));
-  kernel_of(h->kind, 128, true)<<<h->grid, kThreads, h->smem, st>>>(h->args);
+  kernel_of(h->kind, 0, true)<<<h->grid, kThreads, h->smem, st>>>(h->args);
   TNB_LAUNCH_CHECK();
   count_launch();
   set_kernel_name(h->kind == 2 ? "wgmma_chain_tf32" : "wgmma_chain_16");
@@ -771,3 +924,16 @@ int gemm_chain_destroy(void* handle) {
 }
 
 }  // namespace tnb
+
+#ifdef TNB200_CHAIN_PHASES
+// Copy the per-CTA phase accumulators ([kPhaseCtas][kPhases] u64) to host memory, then zero them if `reset`.
+extern "C" TNB200_API int32_t tnb200_chain_phases(unsigned long long* out, int32_t reset) {
+  if (cudaMemcpyFromSymbol(out, tnb::g_chain_phase, sizeof(tnb::g_chain_phase)) != cudaSuccess) return TNB200_ERR_CUDA;
+  if (reset) {
+    void* p = nullptr;
+    if (cudaGetSymbolAddress(&p, tnb::g_chain_phase) != cudaSuccess || cudaMemset(p, 0, sizeof(tnb::g_chain_phase)) != cudaSuccess)
+      return TNB200_ERR_CUDA;
+  }
+  return 0;
+}
+#endif
