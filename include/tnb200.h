@@ -210,7 +210,7 @@ TNB200_API int32_t tnb200_gather(const void* src, const int64_t* idx_dev, void* 
  * contractors/opt_einsum_paths/path_contractors.py:87-90, e.g. the MPS zipper) as ONE persistent launch.
  * Step i is the contraction tnb200_tensordot(a, b, c, ...) would perform; dep_a / dep_b name the earlier step
  * of the chain whose output `c` is this step's operand (or -1 when the operand exists before the launch).
- * Every step must be a tensor-core GEMM addressable in place (M >= 256, N >= 128, 16/32-bit float, one batch
+ * Every step must be a tensor-core GEMM addressable in place (M >= 128, N >= 128, 16/32-bit float, one batch
  * mode shared by all steps); otherwise create() returns TNB200_ERR_UNSUPPORTED with *first_unsupported = the
  * offending step and the caller launches the steps one by one.  create() allocates device tables (not
  * capturable); launch() is stream-ordered and capturable; operand addresses are frozen at create(). */

@@ -785,9 +785,18 @@ struct ChainHandle {
   unsigned grid = 0;
 };
 
-int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, const int* dep_b, void** handle) {
+int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, const int* dep_b, int* first_unsupported,
+                      void** handle) {
   *handle = nullptr;
   if (nsteps < 1) return TNB200_ERR_INVALID;
+  // every step runs in the shared kernel's tiles (M and N of at least 128) over the same samples and dtype
+  for (int i = 0; i < nsteps; ++i) {
+    const GemmProblem& g = probs[i];
+    if (g.M < 128 || g.N < 128 || g.batch != probs[0].batch || g.dtype != probs[0].dtype) {
+      if (first_unsupported) *first_unsupported = i;
+      return TNB200_ERR_UNSUPPORTED;
+    }
+  }
   {
     static int disabled = -1;
     if (disabled < 0) { const char* e = getenv("TNB200_NO_CHAIN"); disabled = (e && e[0] == '1') ? 1 : 0; }
@@ -800,7 +809,7 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
   int64_t sample_bytes = 0;       // largest per-sample footprint of one step: both operands and the result
   for (int i = 0; i < nsteps; ++i) {
     const GemmProblem& g = probs[i];
-    if (g.dtype != dtype || g.batch != batch || g.conjA || g.conjB || g.swapped) return TNB200_ERR_UNSUPPORTED;
+    if (g.conjA || g.conjB || g.swapped) return TNB200_ERR_UNSUPPORTED;
     if (g.dtype != TNB200_F32 && g.dtype != TNB200_F16 && g.dtype != TNB200_BF16) return TNB200_ERR_UNSUPPORTED;
     if (g.c_sn != 1 || g.M >= (1LL << 31) || g.N >= (1LL << 31) || g.K >= (1LL << 31)) return TNB200_ERR_UNSUPPORTED;
     if (dep_a[i] >= i || dep_b[i] >= i) return TNB200_ERR_INVALID;

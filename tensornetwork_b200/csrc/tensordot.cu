@@ -215,15 +215,12 @@ static int dispatch_simt(int dt, const void* A, const void* B, void* C, const Mo
 }
 
 // ------------------------------------------------------------------------------ planner
-struct KMode { int64_t ext, sa, sb; };
-
-// collapse one operand's view of a mode group to "single stride or not"
-static bool single_mode(const ModeList& in, int which, int64_t& ext, int64_t& stride) {
+// collapse one operand's view (stride slot `which`) of a mode group to "single stride or not"
+static bool single_mode(const ModeList& in, int which, int64_t& stride) {
   ModeList m;
   for (int i = 0; i < in.n; ++i) m.push(in.ext[i], which == 0 ? in.s0[i] : (which == 1 ? in.s1[i] : in.s2[i]));
   merge_modes(m, 1);
   if (m.n > 1) return false;
-  ext = m.n ? m.ext[0] : 1;
   stride = m.n ? m.s0[0] : 0;
   return true;
 }
@@ -240,10 +237,10 @@ static ModeList order_k(const ModeList& mK, int by) {
   return r;
 }
 
-// Pack a (batch, free, K) view of one operand into a contiguous row-major [batch, free, K]
-// scratch buffer with the strided-copy kernel (the only place a transpose is materialised).
-static int pack_operand(int dt, const void* src, const ModeList& mB, int wb, const ModeList& mF,
-                        const ModeList& mK, int wk, void** out, int64_t* pitch, cudaStream_t st) {
+// Pack a (batch, free, K) view of operand `w` (its strides: slot w of mB and mK, slot 0 of mF) into a contiguous
+// row-major [batch, free, K] scratch buffer with the strided-copy kernel (the only place a transpose is materialised).
+static int pack_operand(int dt, const void* src, int w, const ModeList& mB, const ModeList& mF, const ModeList& mK,
+                        void** out, int64_t* pitch, cudaStream_t st) {
   tnb200_tensor_t s, d;
   s.data = const_cast<void*>(src); s.dtype = dt; d.dtype = dt;
   int nd = 0;
@@ -256,7 +253,7 @@ static int pack_operand(int dt, const void* src, const ModeList& mB, int wb, con
     }
     return true;
   };
-  if (!add(mB, wb) || !add(mF, 0) || !add(mK, wk)) {
+  if (!add(mB, w) || !add(mF, 0) || !add(mK, w)) {
     set_error("tensordot: too many modes to pack");
     return TNB200_ERR_UNSUPPORTED;
   }
@@ -284,16 +281,11 @@ static int pack_operand(int dt, const void* src, const ModeList& mB, int wb, con
   return copy_strided(&s, &d, 0, st);
 }
 
-}  // namespace tnb
-
-using namespace tnb;
-
-namespace tnb {
 // Validate a contraction request and classify its axes into batch / free-A (M) / free-B (N) / contracted (K)
 // mode lists (np.tensordot output order: batch axes, free axes of a, free axes of b).
-int build_modes(const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200_tensor_t* c, int32_t naxes,
-                const int32_t* axes_a, const int32_t* axes_b, int32_t nbatch, const int32_t* batch_a,
-                const int32_t* batch_b, ModeList& mB, ModeList& mM, ModeList& mN, ModeList& mK) {
+static int build_modes(const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200_tensor_t* c, int32_t naxes,
+                       const int32_t* axes_a, const int32_t* axes_b, int32_t nbatch, const int32_t* batch_a,
+                       const int32_t* batch_b, ModeList& mB, ModeList& mM, ModeList& mN, ModeList& mK) {
   TNB_REQUIRE(valid_tensor(a) && valid_tensor(b) && valid_tensor(c), TNB200_ERR_INVALID,
               "tensordot: invalid tensor descriptor");
   TNB_REQUIRE(a->dtype == b->dtype && a->dtype == c->dtype, TNB200_ERR_DTYPE,
@@ -347,48 +339,68 @@ int build_modes(const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200
   return 0;
 }
 
-// Lower a contraction to a GEMM whose operands are BOTH addressable in place by the TMA / wgmma path
-// (no repack, no skinny / thin special case).  Used by the chained-GEMM planner (gemm_chain.cu).
-int plan_inplace_gemm(const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200_tensor_t* c, int32_t naxes,
-                      const int32_t* axes_a, const int32_t* axes_b, int32_t nbatch, const int32_t* batch_a,
-                      const int32_t* batch_b, GemmProblem& g) {
-  ModeList mB, mM, mN, mK;
-  int rc = build_modes(a, b, c, naxes, axes_a, axes_b, nbatch, batch_a, batch_b, mB, mM, mN, mK);
-  if (rc) return rc;
-  const int dt = a->dtype;
-  if (dt != TNB200_F32 && dt != TNB200_F16 && dt != TNB200_BF16) return TNB200_ERR_UNSUPPORTED;
-  const int64_t M = mM.total(), N = mN.total(), K = mK.total(), Bt = mB.total();
-  if (M == 0 || N == 0 || Bt == 0 || K == 0) return TNB200_ERR_UNSUPPORTED;
-  ModeList gB = mB, gM = mM, gN = mN;
-  merge_modes(gB, 3); merge_modes(gM, 2); merge_modes(gN, 2);
-  if (gB.n > 1) return TNB200_ERR_UNSUPPORTED;
-  int64_t cm_ext, cm_s, cn_ext, cn_s;
-  ModeList cM, cN;
-  for (int i = 0; i < gM.n; ++i) cM.push(gM.ext[i], gM.s1[i]);
-  for (int i = 0; i < gN.n; ++i) cN.push(gN.ext[i], gN.s1[i]);
-  if (!(single_mode(cM, 0, cm_ext, cm_s) && single_mode(cN, 0, cn_ext, cn_s))) return TNB200_ERR_UNSUPPORTED;
+// A contraction lowered to a GEMM: g.A / g.B address the operands in place under the joint order `ko` of the
+// contracted modes, and inA / inB tell whether the kernel can take them so (otherwise they must be repacked).
+struct Lowering {
+  GemmProblem g;
+  ModeList ko;
+  bool inA = false, inB = false;
+};
+
+// Lower a contraction, given its merged batch / M / N groups and unmerged K modes, to a GEMM.  C must be one stride
+// per group.  K is ordered by A's strides (candidate 0) or by B's (candidate 1) and merged jointly, so that both
+// operands walk it in the same steps; the candidate under which more operands are addressable in place wins, the
+// earlier one on a tie.  In place means TMA-addressable for 16/32-bit and one mode per group for f64 (DMMA).
+static int lower_gemm(int dt, const void* A, const void* B, void* C, const ModeList& gB, const ModeList& gM,
+                      const ModeList& gN, const ModeList& mK, Lowering& L) {
+  GemmProblem& g = L.g;
   g = GemmProblem();
-  g.dtype = dt; g.M = M; g.N = N; g.K = K; g.batch = Bt;
-  g.C = c->data; g.c_sm = cm_s; g.c_sn = cn_s; g.c_sb = gB.n ? gB.s2[0] : 0;
+  if (gB.n > 1 || !single_mode(gM, 1, g.c_sm) || !single_mode(gN, 1, g.c_sn)) return TNB200_ERR_UNSUPPORTED;
+  g.dtype = dt; g.M = gM.total(); g.N = gN.total(); g.K = mK.total(); g.batch = gB.total();
+  g.C = C; g.c_sb = gB.n ? gB.s2[0] : 0;
+  auto in_place = [&](const OperandView& v, int64_t ext_f) {
+    return dt == TNB200_F64 ? v.simple() : tma_view_ok(dt, v, ext_f, g.K, g.batch);
+  };
+  int best = -1;
   for (int cand = 0; cand < 2; ++cand) {
     ModeList ko = order_k(mK, cand);
     merge_modes(ko, 2);
     if (ko.n > 4 || gM.n > 4 || gN.n > 4) continue;
     OperandView va, vb;
-    va.ptr = a->data; vb.ptr = b->data;
+    va.ptr = A; vb.ptr = B;
     va.nF = gM.n; for (int i = 0; i < gM.n; ++i) { va.fe[i] = gM.ext[i]; va.fs[i] = gM.s0[i]; }
     vb.nF = gN.n; for (int i = 0; i < gN.n; ++i) { vb.fe[i] = gN.ext[i]; vb.fs[i] = gN.s0[i]; }
     va.nK = vb.nK = ko.n;
     for (int i = 0; i < ko.n; ++i) { va.ke[i] = vb.ke[i] = ko.ext[i]; va.ks[i] = ko.s0[i]; vb.ks[i] = ko.s1[i]; }
     va.sb = gB.n ? gB.s0[0] : 0; vb.sb = gB.n ? gB.s1[0] : 0;
-    if (tma_view_ok(dt, va, M, K, Bt) && tma_view_ok(dt, vb, N, K, Bt)) {
-      g.A = va; g.B = vb;
-      return 0;
-    }
+    const bool okA = in_place(va, g.M), okB = in_place(vb, g.N);
+    if (okA + okB > best) { best = okA + okB; L.ko = ko; g.A = va; g.B = vb; L.inA = okA; L.inB = okB; }
   }
-  return TNB200_ERR_UNSUPPORTED;
+  return best < 0 ? TNB200_ERR_UNSUPPORTED : 0;
 }
+
+// Plan one step of a chained launch: a 16/32-bit GEMM whose operands are both addressable in place (no repack,
+// no thin / skinny special case).
+static int plan_inplace_gemm(const tnb200_chain_step_t& s, GemmProblem& g) {
+  ModeList mB, mM, mN, mK;
+  int rc = build_modes(&s.a, &s.b, &s.c, s.naxes, s.axes_a, s.axes_b, s.nbatch, s.batch_a, s.batch_b, mB, mM, mN, mK);
+  if (rc) return rc;
+  const int dt = s.a.dtype;
+  if (dt != TNB200_F32 && dt != TNB200_F16 && dt != TNB200_BF16) return TNB200_ERR_UNSUPPORTED;
+  if (mM.total() == 0 || mN.total() == 0 || mB.total() == 0 || mK.total() == 0) return TNB200_ERR_UNSUPPORTED;
+  ModeList gB = mB, gM = mM, gN = mN;
+  merge_modes(gB, 3); merge_modes(gM, 2); merge_modes(gN, 2);
+  Lowering L;
+  rc = lower_gemm(dt, s.a.data, s.b.data, s.c.data, gB, gM, gN, mK, L);
+  if (rc) return rc;
+  if (!(L.inA && L.inB)) return TNB200_ERR_UNSUPPORTED;
+  g = L.g;
+  return 0;
+}
+
 }  // namespace tnb
+
+using namespace tnb;
 
 extern "C" int32_t tnb200_tensordot(const tnb200_tensor_t* a, const tnb200_tensor_t* b,
                                     const tnb200_tensor_t* c, int32_t naxes, const int32_t* axes_a,
@@ -427,98 +439,41 @@ extern "C" int32_t tnb200_tensordot(const tnb200_tensor_t* a, const tnb200_tenso
                          !(dt == TNB200_F32 && math == (TNB200_MATH_STRICT >> 4)) &&
                          (double)M * (double)N * (double)K * (double)Bt >= 32768.0 && gB.n <= 1 &&
                          !(M <= 64 && N <= 64 && Bt * 2 <= num_sms() && K >= 8192);   // skinny, long K: split-K SIMT
-  if (want_gemm) {
-    int64_t cm_ext, cm_s, cn_ext, cn_s;
-    ModeList cM, cN;
-    for (int i = 0; i < gM.n; ++i) cM.push(gM.ext[i], gM.s1[i]);
-    for (int i = 0; i < gN.n; ++i) cN.push(gN.ext[i], gN.s1[i]);
-    bool c_ok = single_mode(cM, 0, cm_ext, cm_s) && single_mode(cN, 0, cn_ext, cn_s);
-    if (c_ok) {
-      GemmProblem g;
-      g.dtype = dt; g.M = M; g.N = N; g.K = K; g.batch = Bt; g.conjA = conjA; g.conjB = conjB; g.math = math;
-      g.C = c->data; g.c_sm = cm_s; g.c_sn = cn_s; g.c_sb = gB.n ? gB.s2[0] : 0;
-      // Build both operand views under a common ordering of the contracted modes; try the order
-      // that sorts them by A's strides and the one that sorts by B's, keep the one under which
-      // more operands are addressable in place (TMA for 16/32-bit, 2-stride cp.async for f64).
-      auto make_views = [&](int cand, OperandView& va, OperandView& vb) -> bool {
-        ModeList ko = order_k(mK, cand);
-        merge_modes(ko, 2);                 // joint merge keeps A's and B's k orders identical
-        if (ko.n > 4 || gM.n > 4 || gN.n > 4) return false;
-        va = OperandView(); vb = OperandView();
-        va.ptr = a->data; vb.ptr = b->data;
-        va.nF = gM.n; for (int i = 0; i < gM.n; ++i) { va.fe[i] = gM.ext[i]; va.fs[i] = gM.s0[i]; }
-        vb.nF = gN.n; for (int i = 0; i < gN.n; ++i) { vb.fe[i] = gN.ext[i]; vb.fs[i] = gN.s0[i]; }
-        va.nK = vb.nK = ko.n;
-        for (int i = 0; i < ko.n; ++i) { va.ke[i] = vb.ke[i] = ko.ext[i]; va.ks[i] = ko.s0[i]; vb.ks[i] = ko.s1[i]; }
-        va.sb = gB.n ? gB.s0[0] : 0; vb.sb = gB.n ? gB.s1[0] : 0;
-        return true;
-      };
-      auto view_ok = [&](const OperandView& v, int64_t ef) -> bool {
-        if (dt == TNB200_F64) return v.simple();
-        return tma_view_ok(dt, v, ef, K, Bt);
-      };
-      int best = -1, best_score = -1; bool bestA = false, bestB = false;
-      OperandView va, vb;
-      for (int cand = 0; cand < 2; ++cand) {
-        OperandView xa, xb;
-        if (!make_views(cand, xa, xb)) continue;
-        bool okA = view_ok(xa, M), okB = view_ok(xb, N);
-        int score = (okA ? 1 : 0) + (okB ? 1 : 0);
-        if (score > best_score) { best_score = score; best = cand; bestA = okA; bestB = okB; va = xa; vb = xb; }
+  Lowering L;
+  if (want_gemm && lower_gemm(dt, a->data, b->data, c->data, gB, gM, gN, mK, L) == 0) {
+    GemmProblem& g = L.g;
+    g.conjA = conjA; g.conjB = conjB; g.math = math;
+    void* pk[2] = {nullptr, nullptr};
+    int64_t pitch[2] = {0, 0};
+    // Operand w (0 = A, 1 = B) as a contiguous K-major [batch, free, K] matrix, K in the order `ko`; packed on first
+    // use.  Its K is one mode, or split like `split`, the partner's in-place view, so that both walk K alike.
+    auto packed = [&](int w, const OperandView* split, OperandView& v) -> int {
+      if (!pk[w]) {
+        int rc = pack_operand(dt, w ? b->data : a->data, w, gB, w ? gN : gM, L.ko, &pk[w], &pitch[w], st);
+        if (rc) return rc;
       }
-      if (best >= 0) {
-        ModeList ko = order_k(mK, best);
-        merge_modes(ko, 2);
-        void *packA = nullptr, *packB = nullptr;
-        int rc = 0;
-        if (!bestA) {   // repack A as a contiguous K-major [batch, M, K] matrix (k in the common order)
-          int64_t kp = K;
-          rc = pack_operand(dt, a->data, gB, 0, gM, ko, 0, &packA, &kp, st);
-          va = OperandView(); va.ptr = packA; va.nF = 1; va.fe[0] = M; va.fs[0] = kp; va.nK = 1; va.ke[0] = K; va.ks[0] = 1; va.sb = M * kp;
-        }
-        if (rc == 0 && !bestB) {
-          ModeList nB;  // free modes of B with B strides in slot 0
-          for (int i = 0; i < gN.n; ++i) nB.push(gN.ext[i], gN.s0[i]);
-          int64_t kp = K;
-          rc = pack_operand(dt, b->data, gB, 1, nB, ko, 1, &packB, &kp, st);
-          vb = OperandView(); vb.ptr = packB; vb.nF = 1; vb.fe[0] = N; vb.fs[0] = kp; vb.nK = 1; vb.ke[0] = K; vb.ks[0] = 1; vb.sb = N * kp;
-        }
-        if (rc == 0) {
-          // a packed operand still contracts over ALL of K with one stride: collapse the other
-          // operand's view only if it is also single-mode; otherwise both keep `ko`'s mode split
-          if ((!bestA || !bestB) && (va.nK != vb.nK)) {
-            // the in-place operand has several k modes but the packed one has a single merged mode:
-            // give the packed operand the same split (contiguous, so strides are products)
-            OperandView& pk = !bestA ? va : vb;
-            const OperandView& ip = !bestA ? vb : va;
-            pk.nK = ip.nK;
-            int64_t st_ = 1;
-            for (int i = ip.nK - 1; i >= 0; --i) { pk.ke[i] = ip.ke[i]; pk.ks[i] = st_; st_ *= ip.ke[i]; }
-          }
-          g.A = va; g.B = vb;
-          rc = (dt == TNB200_F64) ? gemm_dmma_f64(g, st) : gemm_wgmma(g, st);
-          if (rc == TNB200_ERR_UNSUPPORTED && (bestA || bestB) && !(packA && packB)) {
-            // in-place addressing was rejected at encode time (tile-size dependent): repack everything
-            if (!packA) {
-              int64_t kp = K;
-              rc = pack_operand(dt, a->data, gB, 0, gM, ko, 0, &packA, &kp, st);
-              va = OperandView(); va.ptr = packA; va.nF = 1; va.fe[0] = M; va.fs[0] = kp; va.nK = 1; va.ke[0] = K; va.ks[0] = 1; va.sb = M * kp;
-            } else { va.nK = 1; va.ke[0] = K; va.ks[0] = 1; }
-            if ((rc == 0 || rc == TNB200_ERR_UNSUPPORTED) && !packB) {
-              ModeList nB;
-              for (int i = 0; i < gN.n; ++i) nB.push(gN.ext[i], gN.s0[i]);
-              int64_t kp = K;
-              rc = pack_operand(dt, b->data, gB, 1, nB, ko, 1, &packB, &kp, st);
-              vb = OperandView(); vb.ptr = packB; vb.nF = 1; vb.fe[0] = N; vb.fs[0] = kp; vb.nK = 1; vb.ke[0] = K; vb.ks[0] = 1; vb.sb = N * kp;
-            } else if (packB) { vb.nK = 1; vb.ke[0] = K; vb.ks[0] = 1; }
-            if (rc == 0) { g.A = va; g.B = vb; rc = (dt == TNB200_F64) ? gemm_dmma_f64(g, st) : gemm_wgmma(g, st); }
-          }
-        }
-        if (packA) ws_free(packA, st);
-        if (packB) ws_free(packB, st);
-        if (rc != TNB200_ERR_UNSUPPORTED) return rc;
-      }
+      const int64_t F = w ? N : M;
+      v = OperandView();
+      v.ptr = pk[w]; v.nF = 1; v.fe[0] = F; v.fs[0] = pitch[w]; v.sb = F * pitch[w];
+      v.nK = split ? split->nK : 1;
+      int64_t s = 1;
+      for (int i = v.nK - 1; i >= 0; --i) { v.ke[i] = split ? split->ke[i] : K; v.ks[i] = s; s *= v.ke[i]; }
+      return 0;
+    };
+    // Attempt 1 addresses in place what it can.  The kernel may still reject the problem (an in-place view when it
+    // encodes the tensor maps for its tile size, or the layout of C); attempt 2 then packs both operands.
+    int rc = 0;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+      const bool keepA = attempt == 0 && L.inA, keepB = attempt == 0 && L.inB;
+      if (!keepA) rc = packed(0, keepB ? &g.B : nullptr, g.A);
+      if (rc == 0 && !keepB) rc = packed(1, keepA ? &g.A : nullptr, g.B);
+      if (rc) break;
+      rc = dt == TNB200_F64 ? gemm_dmma_f64(g, st) : gemm_wgmma(g, st);
+      if (rc != TNB200_ERR_UNSUPPORTED || !(L.inA || L.inB)) break;
     }
+    ws_free(pk[0], st);
+    ws_free(pk[1], st);
+    if (rc != TNB200_ERR_UNSUPPORTED) return rc;
   }
   ModeList gK = mK;
   merge_modes(gK, 2);
@@ -535,22 +490,14 @@ extern "C" int32_t tnb200_chain_create(int32_t nsteps, const tnb200_chain_step_t
   std::vector<int> da((size_t)nsteps), db((size_t)nsteps);
   for (int i = 0; i < nsteps; ++i) {
     const tnb200_chain_step_t& s = steps[i];
-    int rc = plan_inplace_gemm(&s.a, &s.b, &s.c, s.naxes, s.axes_a, s.axes_b, s.nbatch, s.batch_a, s.batch_b, probs[i]);
+    int rc = plan_inplace_gemm(s, probs[i]);
     if (rc) { if (first_unsupported) *first_unsupported = i; return rc; }
     da[i] = s.dep_a; db[i] = s.dep_b;
     TNB_REQUIRE(s.dep_a < i && s.dep_b < i, TNB200_ERR_INVALID, "chain: step %d depends on a later step", i);
     TNB_REQUIRE(s.dep_a < 0 || steps[s.dep_a].c.data == s.a.data, TNB200_ERR_INVALID, "chain: dep_a of step %d does not produce its operand", i);
     TNB_REQUIRE(s.dep_b < 0 || steps[s.dep_b].c.data == s.b.data, TNB200_ERR_INVALID, "chain: dep_b of step %d does not produce its operand", i);
   }
-  // tile-shape eligibility is per step: report the first step the chained kernel cannot take
-  for (int i = 0; i < nsteps; ++i) {
-    const GemmProblem& g = probs[i];
-    if (g.M < 128 || g.N < 128 || g.batch != probs[0].batch || g.dtype != probs[0].dtype) {
-      if (first_unsupported) *first_unsupported = i;
-      return TNB200_ERR_UNSUPPORTED;
-    }
-  }
-  return gemm_chain_create(nsteps, probs.data(), da.data(), db.data(), handle);
+  return gemm_chain_create(nsteps, probs.data(), da.data(), db.data(), first_unsupported, handle);
 }
 extern "C" int32_t tnb200_chain_launch(void* handle, void* stream) { return gemm_chain_launch(handle, (cudaStream_t)stream); }
 extern "C" int32_t tnb200_chain_destroy(void* handle) { return gemm_chain_destroy(handle); }

@@ -64,14 +64,39 @@ def test_batched(dtype):
   assert rel_err(out.to_host(), np.matmul(a, b)) < TOLS[dtype]
 
 
+# (dtype, shape of A, slice of A, shape of B, contracted axes, transposed output, kernel, launches including repacks)
+REPACK_CASES = {
+    # odd leading dimension -> not addressable in place -> one strided-copy repack, then the tensor-core GEMM
+    "a_packed": ("bfloat16", (256, 131), None, (131, 256), ([1], [0]), False, "wgmma_bf16", 2),
+    "b_packed": ("bfloat16", (256, 128), None, (128, 131), ([1], [0]), False, "wgmma_bf16", 2),
+    "both_packed": ("bfloat16", (256, 131), None, (131, 260), ([1], [0]), False, "wgmma_bf16", 3),
+    # A keeps two K modes in place (the slice breaks mergeability); the packed B walks K in the same two modes
+    "k_split": ("bfloat16", (256, 2, 128), np.s_[:, :, :64], (2, 64, 129), ([1, 2], [0, 1]), False, "wgmma_bf16", 2),
+    # DMMA addresses only one mode per group: a two-mode free group is repacked, a two-mode K group repacks both
+    "f64_free_modes": ("float64", (4, 64, 128), np.s_[:, :32, :], (128, 128), ([2], [0]), False, "dmma_f64", 2),
+    "f64_k_modes": ("float64", (128, 4, 64), np.s_[:, :, :32], (4, 32, 128), ([1, 2], [0, 1]), False, "dmma_f64", 3),
+    # the GEMM rejects a column-strided C after A was repacked: B is repacked too (A's copy is reused), then SIMT
+    "rejected_retry": ("bfloat16", (256, 131), None, (131, 256), ([1], [0]), True, "simt", 3),
+}
+
+
 def test_unaligned_operand_falls_back_to_repack():
-  """odd leading dimension -> not TMA addressable -> repacked, still tensor-core, still right."""
+  """operands the GEMM cannot address in place are repacked; the kernel, the launch count and the result are pinned."""
   be = get_backend()
-  rng = np.random.default_rng(24)
-  A, a = _mk(be, rng, (256, 131), "bfloat16")
-  B, b = _mk(be, rng, (131, 256), "bfloat16")
-  out = be.tensordot(A, B, 1)
-  assert rel_err(out.to_host(), a @ b) < TOLS["bfloat16"]
+  for case, (dtype, sa, sl, sb, axes, c_transposed, kern, launches) in REPACK_CASES.items():
+    rng = np.random.default_rng(24)
+    A, a = _mk(be, rng, sa, dtype)
+    B, b = _mk(be, rng, sb, dtype)
+    if sl is not None:
+      A, a = A[sl], a[sl]
+    ref = np.tensordot(a, b, axes)
+    out = None
+    if c_transposed:
+      out = be.transpose(be._new(ref.shape[::-1], A.code))  # pylint: disable=protected-access
+    l0 = _launches(be)
+    out = be._contract(A, B, axes[0], axes[1], [], [], out=out)  # pylint: disable=protected-access
+    assert (be.lib.tnb200_last_kernel().decode(), _launches(be) - l0) == (kern, launches), case
+    assert rel_err(out.to_host(), ref) < TOLS.get(dtype, 1e-12), case
 
 
 def test_linearity_at_flagship_size():
@@ -148,6 +173,30 @@ def test_swap_ab_tiny_m(dtype):
   out = be._contract(Ab, Bb, [1], [2], [0], [0])
   ref = np.einsum("bkpq,bxkcdefghi->bpqxcdefghi", ab, bb)
   assert rel_err(out.to_host(), ref) < TOLS[dtype]
+
+
+def test_chain_names_first_step_below_its_tile():
+  """The chained kernel takes steps of at least 128 x 128: create() reports the first smaller step and makes no handle."""
+  import ctypes
+  from tensornetwork_b200 import _lib as L
+  be = get_backend()
+  rng = np.random.default_rng(28)
+  A0, _ = _mk(be, rng, (256, 256), "bfloat16")
+  B0, _ = _mk(be, rng, (256, 256), "bfloat16")
+  A1, _ = _mk(be, rng, (64, 256), "bfloat16")
+  A2, _ = _mk(be, rng, (128, 64), "bfloat16")
+  C0, C1, C2 = (be._new(s, L.BF16) for s in ((256, 256), (64, 256), (128, 256)))  # pylint: disable=protected-access
+  # C0 = A0 B0, C1 = A1 C0 (M = 64), C2 = A2 C1: every step is addressable in place, only step 1 is below the tile
+  steps = [(A0, B0, C0, -1), (A1, C0, C1, 0), (A2, C1, C2, 1)]
+  arr = (L.ChainStep * len(steps))()
+  for cs, (a, b, c, dep_b) in zip(arr, steps):
+    cs.a, cs.b, cs.c = a.desc(), b.desc(), c.desc()
+    cs.naxes, cs.nbatch = 1, 0
+    cs.axes_a[0], cs.axes_b[0] = 1, 0
+    cs.dep_a, cs.dep_b = -1, dep_b
+  bad, handle = ctypes.c_int32(-1), ctypes.c_void_p()
+  rc = be.lib.tnb200_chain_create(len(steps), arr, ctypes.byref(bad), ctypes.byref(handle))
+  assert (rc, bad.value, handle.value) == (L.ERR_UNSUPPORTED, 1, None)
 
 
 # ------------------------------------------------------------------------------------------------
