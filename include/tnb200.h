@@ -211,9 +211,12 @@ TNB200_API int32_t tnb200_gather(const void* src, const int64_t* idx_dev, void* 
  * Step i is the contraction tnb200_tensordot(a, b, c, ...) would perform; dep_a / dep_b name the earlier step
  * of the chain whose output `c` is this step's operand (or -1 when the operand exists before the launch).
  * Every step must be a tensor-core GEMM addressable in place (M >= 128, N >= 128, 16/32-bit float, one batch
- * mode shared by all steps); otherwise create() returns TNB200_ERR_UNSUPPORTED with *first_unsupported = the
- * offending step and the caller launches the steps one by one.  create() allocates device tables (not
- * capturable); launch() is stream-ordered and capturable; operand addresses are frozen at create(). */
+ * mode shared by all steps, C row-major with 16-byte aligned rows); otherwise create() returns
+ * TNB200_ERR_UNSUPPORTED with *first_unsupported = the first offending step, and the caller can split the run
+ * around it.  When the chain as a whole is declined (TNB200_NO_CHAIN set, too few tiles per step to fill the GPU,
+ * not enough shared memory) create() returns TNB200_ERR_UNSUPPORTED with *first_unsupported = -1 and the caller
+ * launches the steps one by one.  create() allocates device tables (not capturable); launch() is stream-ordered
+ * and capturable; operand addresses are frozen at create(). */
 typedef struct {
   tnb200_tensor_t a, b, c;
   int32_t naxes, nbatch;

@@ -35,8 +35,9 @@ int gemm_wgmma(const GemmProblem& p, cudaStream_t st);     // bf16 / f16 / f32(t
 int gemm_dmma_f64(const GemmProblem& p, cudaStream_t st);  // f64 via mma.sync DMMA
 // Chained GEMMs in one persistent launch (gemm_wgmma.cu): dep_a[i] / dep_b[i] = index of the chain step whose
 // output is step i's operand A / B (or -1).  create() allocates device tables (call it outside stream capture).
-// A step below the kernel's 128 x 128 tile, or with another batch or dtype than step 0, is reported in
-// *first_unsupported (when not null) with TNB200_ERR_UNSUPPORTED.
+// A step the kernel cannot take (below its 128 x 128 tile, another batch or dtype than step 0, a C that is not
+// row-major with 16-byte aligned rows, operands its tensor maps cannot address) is reported in *first_unsupported
+// (when not null) with TNB200_ERR_UNSUPPORTED; a rejection of the chain as a whole leaves it at -1.
 int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, const int* dep_b, int* first_unsupported,
                       void** handle);
 int gemm_chain_launch(void* handle, cudaStream_t st);

@@ -789,13 +789,14 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
                       void** handle) {
   *handle = nullptr;
   if (nsteps < 1) return TNB200_ERR_INVALID;
+  // A step the kernel cannot take is named in *first_unsupported, so that the caller can split the run around it.
+  // Rejections of the chain as a whole (disabled, too few tiles, shared memory) leave it at -1.
+  auto reject = [&](int i, int rc) { if (first_unsupported) *first_unsupported = i; return rc; };
   // every step runs in the shared kernel's tiles (M and N of at least 128) over the same samples and dtype
   for (int i = 0; i < nsteps; ++i) {
     const GemmProblem& g = probs[i];
-    if (g.M < 128 || g.N < 128 || g.batch != probs[0].batch || g.dtype != probs[0].dtype) {
-      if (first_unsupported) *first_unsupported = i;
-      return TNB200_ERR_UNSUPPORTED;
-    }
+    if (g.M < 128 || g.N < 128 || g.batch != probs[0].batch || g.dtype != probs[0].dtype)
+      return reject(i, TNB200_ERR_UNSUPPORTED);
   }
   {
     static int disabled = -1;
@@ -809,17 +810,17 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
   int64_t sample_bytes = 0;       // largest per-sample footprint of one step: both operands and the result
   for (int i = 0; i < nsteps; ++i) {
     const GemmProblem& g = probs[i];
-    if (g.conjA || g.conjB || g.swapped) return TNB200_ERR_UNSUPPORTED;
-    if (g.dtype != TNB200_F32 && g.dtype != TNB200_F16 && g.dtype != TNB200_BF16) return TNB200_ERR_UNSUPPORTED;
-    if (g.c_sn != 1 || g.M >= (1LL << 31) || g.N >= (1LL << 31) || g.K >= (1LL << 31)) return TNB200_ERR_UNSUPPORTED;
+    if (g.conjA || g.conjB || g.swapped) return reject(i, TNB200_ERR_UNSUPPORTED);
+    if (g.dtype != TNB200_F32 && g.dtype != TNB200_F16 && g.dtype != TNB200_BF16) return reject(i, TNB200_ERR_UNSUPPORTED);
+    if (g.c_sn != 1 || g.M >= (1LL << 31) || g.N >= (1LL << 31) || g.K >= (1LL << 31)) return reject(i, TNB200_ERR_UNSUPPORTED);
     if (dep_a[i] >= i || dep_b[i] >= i) return TNB200_ERR_INVALID;
     TcPrep prep;
     int rc = tc_prepare(g, true, prep);
-    if (rc) return rc;
+    if (rc) return reject(i, rc);
     ChainStepDev& sd = steps[i];
     memset(&sd, 0, sizeof(sd));
     rc = encode_output(&sd.tmC, g);
-    if (rc) return rc;
+    if (rc) return reject(i, rc);
     sd.tmA = prep.tmA; sd.tmB = prep.tmB; sd.p = prep.p;
     sd.dep_a = dep_a[i]; sd.dep_b = dep_b[i];
     sd.tiles_per_sample = (int)(prep.p.tiles_m * prep.p.tiles_n);
