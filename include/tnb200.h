@@ -229,6 +229,20 @@ TNB200_API int32_t tnb200_chain_create(int32_t nsteps, const tnb200_chain_step_t
 TNB200_API int32_t tnb200_chain_launch(void* handle, void* stream);
 TNB200_API int32_t tnb200_chain_destroy(void* handle);
 
+/* ---- a RUN of 2..8 thin contractions (the ramp of an MPS contraction: a small matrix, K <= 64, applied to a long
+ * operand) in which step i streams step i - 1's result: ONE persistent launch that reads the first long operand once,
+ * keeps every intermediate on chip and writes only the last step's result, bit-identical to launching the steps one by
+ * one.  Steps are described as for tnb200_chain_create; dep_a / dep_b of step i > 0 name step i - 1 for the long
+ * operand and -1 for the small one, and the `data` of an intermediate result is not used (it may be NULL).  Each
+ * step must take the 16-bit thin layout tnb200_tensordot would launch for it, all in one mode, with the previous
+ * result's long axis innermost (columns) or outermost (rows) in the next long axis; otherwise create() returns
+ * TNB200_ERR_UNSUPPORTED with *first_unsupported = the offending step (-1 when the run is declined as a whole).
+ * create() allocates a device table (not capturable); launch() is stream-ordered and capturable. */
+TNB200_API int32_t tnb200_thin_run_create(int32_t nsteps, const tnb200_chain_step_t* steps, int32_t* first_unsupported,
+                                          void** handle);
+TNB200_API int32_t tnb200_thin_run_launch(void* handle, void* stream);
+TNB200_API int32_t tnb200_thin_run_destroy(void* handle);
+
 #ifdef __cplusplus
 }
 #endif

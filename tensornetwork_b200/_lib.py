@@ -74,6 +74,9 @@ SIGNATURES = {
     "tnb200_chain_create": (_i32, [_i32, ctypes.POINTER(ChainStep), _pi32, ctypes.POINTER(_vp)]),
     "tnb200_chain_launch": (_i32, [_vp, _vp]),
     "tnb200_chain_destroy": (_i32, [_vp]),
+    "tnb200_thin_run_create": (_i32, [_i32, ctypes.POINTER(ChainStep), _pi32, ctypes.POINTER(_vp)]),
+    "tnb200_thin_run_launch": (_i32, [_vp, _vp]),
+    "tnb200_thin_run_destroy": (_i32, [_vp]),
 }
 
 _lib = None

@@ -16,6 +16,11 @@ int tensordot_thin(int dt, const void* A, const void* B, void* C, const ModeList
                    const ModeList& mN, const ModeList& mK, bool allow_tf32, cudaStream_t st);
 int tensordot_skinny(int dt, const void* A, const void* B, void* C, const ModeList& mB, const ModeList& mM,
                      const ModeList& mN, const ModeList& mK, cudaStream_t st);
+int thin_run_create(int dt, int nsteps, const ModeList* mB, const ModeList* mM, const ModeList* mN, const ModeList* mK,
+                    const void* const* A, const void* const* B, void* const* C, const int* dep_a, const int* dep_b,
+                    int* bad, void** handle);
+int thin_run_launch(void* handle, cudaStream_t st);
+int thin_run_destroy(void* handle);
 
 // --------------------------------------------------------------------------- SIMT kernel
 template <typename T>
@@ -501,3 +506,36 @@ extern "C" int32_t tnb200_chain_create(int32_t nsteps, const tnb200_chain_step_t
 }
 extern "C" int32_t tnb200_chain_launch(void* handle, void* stream) { return gemm_chain_launch(handle, (cudaStream_t)stream); }
 extern "C" int32_t tnb200_chain_destroy(void* handle) { return gemm_chain_destroy(handle); }
+
+// ------------------------------------------------------------------------------------------ fused thin runs
+extern "C" int32_t tnb200_thin_run_create(int32_t nsteps, const tnb200_chain_step_t* steps, int32_t* first_unsupported,
+                                          void** handle) {
+  TNB_REQUIRE(nsteps >= 1 && steps && handle, TNB200_ERR_INVALID, "thin run: bad arguments");
+  *handle = nullptr;
+  if (first_unsupported) *first_unsupported = -1;
+  std::vector<ModeList> mB((size_t)nsteps), mM((size_t)nsteps), mN((size_t)nsteps), mK((size_t)nsteps);
+  std::vector<const void*> A((size_t)nsteps), B((size_t)nsteps);
+  std::vector<void*> C((size_t)nsteps);
+  std::vector<int> da((size_t)nsteps), db((size_t)nsteps);
+  for (int i = 0; i < nsteps; ++i) {
+    const tnb200_chain_step_t& s = steps[i];
+    int rc = build_modes(&s.a, &s.b, &s.c, s.naxes, s.axes_a, s.axes_b, s.nbatch, s.batch_a, s.batch_b, mB[i], mM[i],
+                         mN[i], mK[i]);
+    if (rc) { if (first_unsupported) *first_unsupported = i; return rc; }
+    TNB_REQUIRE(s.dep_a < i && s.dep_b < i, TNB200_ERR_INVALID, "thin run: step %d depends on a later step", i);
+    // the same lowering as tnb200_tensordot, so that each step takes the thin layout its own launch would take
+    merge_modes(mB[i], 3); merge_modes(mM[i], 2); merge_modes(mN[i], 2); merge_modes(mK[i], 2);
+    A[i] = s.a.data; B[i] = s.b.data; C[i] = s.c.data;
+    da[i] = s.dep_a; db[i] = s.dep_b;
+  }
+  int bad = -1;
+  const int rc = thin_run_create(steps[0].a.dtype, nsteps, mB.data(), mM.data(), mN.data(), mK.data(), A.data(), B.data(),
+                                 C.data(), da.data(), db.data(), &bad, handle);
+  if (rc && first_unsupported) *first_unsupported = bad;
+  return rc;
+}
+extern "C" int32_t tnb200_thin_run_launch(void* handle, void* stream) {
+  TNB_REQUIRE(handle, TNB200_ERR_INVALID, "thin run: null handle");
+  return thin_run_launch(handle, (cudaStream_t)stream);
+}
+extern "C" int32_t tnb200_thin_run_destroy(void* handle) { return thin_run_destroy(handle); }

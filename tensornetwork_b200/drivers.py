@@ -434,20 +434,57 @@ def find_chains(steps, n_inputs, min_len=2):
   return runs
 
 
-class _Chain:
-  """A created chained launch: owns the library handle; `steps` are the plan step indices it covers."""
+def find_thin_runs(steps, n_inputs, res_slot, shapes, exclude=(), max_len=8):
+  """Runs of thin contraction steps linked by dependency (not by index: the ramps of an MPS contraction interleave):
+  candidates for one fused launch (tnb200_thin_run_create).  A step is thin when it contracts at most 64 elements;
+  step s continues into step u when u is the only consumer of s's result, that result is not the network's result and
+  it is u's long operand (larger than u's other operand).  `shapes` are the slot shapes of plan_shapes; steps in
+  `exclude` take no part.  Returns lists of at most `max_len` step indices, each at least two long."""
+  def thin(i):
+    st = steps[i]
+    if i in exclude or st[0] not in ("tensordot", "batched"):
+      return False
+    return int(np.prod([shapes[st[1]][a] for a in st[3]] or [1])) <= 64
+  users = {}
+  for i, st in enumerate(steps):
+    for x in ((st[1], st[2]) if st[0] != "transpose" else (st[1],)):
+      users.setdefault(x, []).append(i)
+  nxt, has_prev = {}, set()
+  for s in range(len(steps)):
+    out = n_inputs + s
+    u = users.get(out, [])
+    if not thin(s) or out == res_slot or len(u) != 1 or not thin(u[0]):
+      continue
+    other = steps[u[0]][2] if steps[u[0]][1] == out else steps[u[0]][1]
+    if other != out and np.prod(shapes[out]) > np.prod(shapes[other]):
+      nxt[s] = u[0]
+      has_prev.add(u[0])
+  runs = []
+  for s in sorted(nxt):
+    if s in has_prev:
+      continue
+    path = [s]
+    while path[-1] in nxt:
+      path.append(nxt[path[-1]])
+    runs += [path[i:i + max_len] for i in range(0, len(path), max_len) if len(path[i:i + max_len]) >= 2]
+  return runs
 
-  def __init__(self, backend, handle, step_ids):
-    self.backend, self.handle, self.steps = backend, handle, list(step_ids)
+
+class _Chain:
+  """A created chained launch (api "chain") or fused thin run (api "thin_run"): owns the library handle; `steps` are
+  the plan step indices it covers."""
+
+  def __init__(self, backend, handle, step_ids, api="chain"):
+    self.backend, self.handle, self.steps, self.api = backend, handle, list(step_ids), api
 
   def launch(self):
     from . import _lib as L  # pylint: disable=import-outside-toplevel
-    L.check(self.backend.lib.tnb200_chain_launch(self.handle, self.backend._stream()))  # pylint: disable=protected-access
+    L.check(getattr(self.backend.lib, "tnb200_%s_launch" % self.api)(self.handle, self.backend._stream()))  # pylint: disable=protected-access
 
   def __del__(self):
     try:
       if self.handle:
-        self.backend.lib.tnb200_chain_destroy(self.handle)
+        getattr(self.backend.lib, "tnb200_%s_destroy" % self.api)(self.handle)
         self.handle = None
     except Exception:  # pylint: disable=broad-except
       pass
@@ -590,10 +627,7 @@ class CompiledNetwork:
       pending = []            # the chained kernel computes fp32 as TF32: strict fp32 stays on per-step launches
     if be.math_mode == L.MATH_SIMT:
       pending = []
-    while pending:
-      run = pending.pop(0)
-      if len(run) < 2:
-        continue
+    def step_array(run):
       pos = {sid: k for k, sid in enumerate(run)}
       arr = (L.ChainStep * len(run))()
       for k, sid in enumerate(run):
@@ -617,27 +651,48 @@ class CompiledNetwork:
         # operands that are (views of) results of earlier steps of this run
         cs.dep_a = self._producer(st[1], n_in, pos)
         cs.dep_b = self._producer(st[2], n_in, pos)
-      handle = ctypes.c_void_p()
-      bad = ctypes.c_int32(-1)
-      rc = be.lib.tnb200_chain_create(len(run), arr, ctypes.byref(bad), ctypes.byref(handle))
-      if rc == 0:
-        ch = _Chain(be, handle, run)
-        self.chains.append(ch)
-        for sid in run:
-          chain_of[sid] = ch
-      elif rc == L.ERR_UNSUPPORTED:
-        k = bad.value if bad.value >= 0 else 0      # split the run around the step the kernel cannot take
-        pending[:0] = [run[:k], run[k + 1:]]
-      else:
-        L.check(rc)
+      return arr
+
+    def create(api, pending):
+      while pending:
+        run = pending.pop(0)
+        if len(run) < 2:
+          continue
+        handle = ctypes.c_void_p()
+        bad = ctypes.c_int32(-1)
+        rc = getattr(be.lib, "tnb200_%s_create" % api)(len(run), step_array(run), ctypes.byref(bad), ctypes.byref(handle))
+        if rc == 0:
+          ch = _Chain(be, handle, run, api)
+          self.chains.append(ch)
+          for sid in run:
+            chain_of[sid] = ch
+        elif rc == L.ERR_UNSUPPORTED:
+          k = bad.value if bad.value >= 0 else 0      # split the run around the step the kernel cannot take
+          pending[:0] = [run[:k], run[k + 1:]]
+        else:
+          L.check(rc)
+    create("chain", pending)
+    # fused thin runs (16-bit only) among the steps no chain took; their intermediates stay on chip, so their
+    # buffers are released
+    thin_pending = [] if be.math_mode == L.MATH_SIMT else find_thin_runs(self.steps, n_in, self.res_slot, shp,
+                                                                         exclude=set(chain_of))
+    create("thin_run", thin_pending)
+    for ch in self.chains:
+      if ch.api == "thin_run":
+        for sid in ch.steps[:-1]:
+          vals[n_in + sid] = None
     nodes, seen = [], set()
     for i, st in enumerate(self.steps):
       ch = chain_of.get(i)
       if ch is None:
         nodes.append(("step", i))
+      elif ch.api == "thin_run":
+        # at its last step: the small operands of its steps may come from steps between its first and last
+        if i == ch.steps[-1]:
+          nodes.append((ch.api, ch))
       elif id(ch) not in seen:
         seen.add(id(ch))
-        nodes.append(("chain", ch))
+        nodes.append((ch.api, ch))
     self._nodes = nodes
 
   def _producer(self, slot, n_in, pos):
@@ -657,11 +712,13 @@ class CompiledNetwork:
     for sid in node[1].steps:
       st = self.steps[sid]
       ins += [x for x in (st[1], st[2]) if x not in outs]
+    if node[0] == "thin_run":
+      outs = outs[-1:]                  # the run's intermediates never leave the chip
     return ins, outs
 
   def _launch_node(self, node):
     be, n_in, vals = self.backend, len(self.inputs), self._vals
-    if node[0] == "chain":
+    if node[0] in ("chain", "thin_run"):
       node[1].launch()
       return
     st = self.steps[node[1]]
