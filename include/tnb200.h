@@ -213,7 +213,7 @@ TNB200_API int32_t tnb200_gather(const void* src, const int64_t* idx_dev, void* 
  * Every step must be a tensor-core GEMM addressable in place (M >= 128, N >= 128, 16/32-bit float, one batch
  * mode shared by all steps, C row-major with 16-byte aligned rows); otherwise create() returns
  * TNB200_ERR_UNSUPPORTED with *first_unsupported = the first offending step, and the caller can split the run
- * around it.  When the chain as a whole is declined (TNB200_NO_CHAIN set, too few tiles per step to fill the GPU,
+ * around it.  When the chain as a whole is declined (too few tiles per step to fill the GPU,
  * not enough shared memory) create() returns TNB200_ERR_UNSUPPORTED with *first_unsupported = -1 and the caller
  * launches the steps one by one.  create() allocates device tables (not capturable); launch() is stream-ordered
  * and capturable; operand addresses are frozen at create(). */

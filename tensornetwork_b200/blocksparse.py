@@ -16,7 +16,6 @@ per (charges, flows, order, partition) signature on the host (pure integer work,
 checked bit-exactly against the reference's maps in tests/) and ALL sectors run in ONE launch
 of the grouped kernel `tnb200_blocksparse_tensordot`.
 """
-import os
 import numpy as np
 from . import _lib as L
 from . import tensor as T
@@ -405,15 +404,9 @@ def tensordot(a, b, axes):
   # matrix views: A = (free_a | axes_a), B = (axes_b | free_b), C = (free_a | free_b)
   order_a = [a.order[i] for i in free_a] + [a.order[i] for i in axes_a]
   order_b = [b.order[i] for i in axes_b] + [b.order[i] for i in free_b]
-  host_maps = os.environ.get("TNB200_BS_HOST_MAPS", "0") == "1"       # measurement / debugging knob: numpy-built maps
-  if host_maps:
-    qa, da, ma = _sector_maps(a.indices, order_a, len(free_a))
-    qb, db, mb = _sector_maps(b.indices, order_b, len(axes_b))
-    qc, dc, mc = _sector_maps(out_indices, list(range(len(out_indices))), len(free_a))
-  else:
-    qa, da, ma, oa = _device_sector_maps(be, a.indices, order_a, len(free_a))
-    qb, db, mb, ob = _device_sector_maps(be, b.indices, order_b, len(axes_b))
-    qc, dc, mc, oc = _device_sector_maps(be, out_indices, list(range(len(out_indices))), len(free_a))
+  qa, da, ma, oa = _device_sector_maps(be, a.indices, order_a, len(free_a))
+  qb, db, mb, ob = _device_sector_maps(be, b.indices, order_b, len(axes_b))
+  qc, dc, mc, oc = _device_sector_maps(be, out_indices, list(range(len(out_indices))), len(free_a))
   nnz_c = BlockSparseTensor._nnz(out_indices)  # pylint: disable=protected-access
   c_data = be.zeros((nnz_c,), a.data.dtype)      # blocksparsetensor.py:1088: zero-initialised
   mod = a.indices[0].modulus if a.indices else None
@@ -439,21 +432,11 @@ def tensordot(a, b, axes):
     torch = be.torch
     dims = np.array([[m_, k_, n_] for (_, _, _, m_, k_, n_) in sect], dtype=np.int64)
     up = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(be.device)
-    if host_maps:
-      def cat(maps, which):
-        arrs = [maps[sc[which]] for sc in sect]
-        off = np.zeros(len(arrs) + 1, dtype=np.int64)
-        off[1:] = np.cumsum([x.shape[0] for x in arrs])
-        return up(np.concatenate(arrs)), off
-      am, ao = cat(ma, 0)
-      bm, bo = cat(mb, 1)
-      cm, co = cat(mc, 2)
-    else:
-      # the device maps hold every sector of their tensor; a contraction sector starts at that sector's offset
-      am, ao = ma, np.array([oa[sc[0]] for sc in sect] + [0], dtype=np.int64)
-      bm, bo = mb, np.array([ob[sc[1]] for sc in sect] + [0], dtype=np.int64)
-      cm, co = mc, np.array([oc[sc[2]] for sc in sect] + [0], dtype=np.int64)
-    dev = dict(dims=up(dims), am=am, ao=up(ao), bm=bm, bo=up(bo), cm=cm, co=up(co),
+    # the device maps hold every sector of their tensor; a contraction sector starts at that sector's offset
+    ao = np.array([oa[sc[0]] for sc in sect] + [0], dtype=np.int64)
+    bo = np.array([ob[sc[1]] for sc in sect] + [0], dtype=np.int64)
+    co = np.array([oc[sc[2]] for sc in sect] + [0], dtype=np.int64)
+    dev = dict(dims=up(dims), am=ma, ao=up(ao), bm=mb, bo=up(bo), cm=mc, co=up(co),
                max_m=int(dims[:, 0].max()), max_n=int(dims[:, 2].max()), nsect=len(sect),
                keep=(ma, mb, mc), flops=float(2 * (dims[:, 0] * dims[:, 1] * dims[:, 2]).sum()))
     _MAP_CACHE[key] = dev

@@ -7,7 +7,6 @@
 // unavoidable gather), multiplies, and scatters C through its map.  Sectors at the BASELINE
 // sizes are tiny (2..66 rows), so this is latency/HBM-bound: no tensor cores, 32x32 tiles.
 #include "common.cuh"
-#include <stdlib.h>
 
 namespace tnb {
 
@@ -199,7 +198,7 @@ extern "C" int32_t tnb200_blocksparse_tensordot(const void* a_data, const void* 
   cudaStream_t st = (cudaStream_t)stream;
   set_kernel_name("blocksparse_grouped");
   const bool cj = conj_b && dtype_is_complex(dtype);
-  if (dtype == TNB200_F64 && max_m >= 48 && max_n >= 48 && !(getenv("TNB200_BS_SIMT") && getenv("TNB200_BS_SIMT")[0] == '1')) {
+  if (dtype == TNB200_F64 && max_m >= 48 && max_n >= 48) {
     const int tiles_m = (int)((max_m + DT_ - 1) / DT_), tiles_n = (int)((max_n + DT_ - 1) / DT_);
     blocksparse_dmma_kernel<<<dim3((unsigned)(tiles_m * tiles_n), (unsigned)nsect), 256, 0, st>>>(
         (const double*)a_data, (const double*)b_data, (double*)c_data, (const long long*)dims_dev, (const long long*)a_map_dev,

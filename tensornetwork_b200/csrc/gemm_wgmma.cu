@@ -790,18 +790,13 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
   *handle = nullptr;
   if (nsteps < 1) return TNB200_ERR_INVALID;
   // A step the kernel cannot take is named in *first_unsupported, so that the caller can split the run around it.
-  // Rejections of the chain as a whole (disabled, too few tiles, shared memory) leave it at -1.
+  // Rejections of the chain as a whole (too few tiles, shared memory) leave it at -1.
   auto reject = [&](int i, int rc) { if (first_unsupported) *first_unsupported = i; return rc; };
   // every step runs in the shared kernel's tiles (M and N of at least 128) over the same samples and dtype
   for (int i = 0; i < nsteps; ++i) {
     const GemmProblem& g = probs[i];
     if (g.M < 128 || g.N < 128 || g.batch != probs[0].batch || g.dtype != probs[0].dtype)
       return reject(i, TNB200_ERR_UNSUPPORTED);
-  }
-  {
-    static int disabled = -1;
-    if (disabled < 0) { const char* e = getenv("TNB200_NO_CHAIN"); disabled = (e && e[0] == '1') ? 1 : 0; }
-    if (disabled) return TNB200_ERR_UNSUPPORTED;
   }
   const int dtype = probs[0].dtype;
   const int64_t batch = probs[0].batch;

@@ -9,7 +9,6 @@
 #include "common.cuh"
 #include "cplx.cuh"
 #include <math.h>
-#include <stdlib.h>
 
 namespace tnb {
 
@@ -503,12 +502,11 @@ extern "C" int32_t tnb200_qr(const tnb200_tensor_t* a, const tnb200_tensor_t* q,
   set_kernel_name("qr_householder");
   cudaStream_t st = (cudaStream_t)stream;
   if (a->dtype == TNB200_F64) {
-    // blocked path: the panel's rows must fit the shared memory of an 8-CTA cluster (m <= ~6500); TNB200_QR_ALGO=columns keeps the
+    // blocked path: the panel's rows must fit the shared memory of an 8-CTA cluster (m <= ~6500); otherwise the
     // one-launch-per-column kernels
-    const char* algo = getenv("TNB200_QR_ALGO");
     const int64_t rl = (m + QCL - 1) / QCL;
     const bool fits = sizeof(double) * ((size_t)QB * (rl + 2) + 2 * QCL * 64 + 128 + QB + QB * (QB + 1)) + 16 <= 226 * 1024;
-    if (fits && k >= 16 && !(algo && !strcmp(algo, "columns"))) { set_kernel_name("qr_blocked_wy"); return qr_blocked_f64(a, q, r, non_negative_diagonal, st); }
+    if (fits && k >= 16) { set_kernel_name("qr_blocked_wy"); return qr_blocked_f64(a, q, r, non_negative_diagonal, st); }
     return qr_real<double>(a, q, r, non_negative_diagonal, st);
   }
   if (a->dtype == TNB200_C128) return qr_real<zd>(a, q, r, non_negative_diagonal, st);

@@ -2,7 +2,7 @@
 // count of decompositions.svd (backends/numpy/decompositions.py:21-74; LAPACK gesdd there).
 //
 // The matrix is copied once into column-contiguous working storage W (tall: rows >= cols; a wide
-// input is handled through its transpose).  Columns are grouped in blocks of SB; a sweep visits
+// input is handled through its transpose).  Columns are grouped in blocks of SB = 16; a sweep visits
 // every block pair in a round-robin tournament (nb-1 rounds of nb/2 disjoint pairs, all pairs of
 // a round processed concurrently):
 //   1. gram   : G = [W_I W_J]^T [W_I W_J]           (2SB x 2SB per pair, split over row chunks)
@@ -14,20 +14,16 @@
 #include "common.cuh"
 #include "cplx.cuh"
 #include <math.h>
-#include <stdlib.h>
 #include <vector>
 
 namespace tnb {
 
 int copy_strided(const tnb200_tensor_t* src, const tnb200_tensor_t* dst, int conj, cudaStream_t st);
 
-// Block width SB (columns per block; a pair rotates PB = 2 SB columns) is a template parameter: 16 is the default,
-// 32 an experiment (see svd_dispatch): every round streams W and V through HBM once, and doubling the block width
-// halves the number of rounds per sweep, but the Gram eigenproblem grows to 64 x 64 (still one CTA).
-template <int SB> struct Geo {
-  static constexpr int PB = 2 * SB;
-  static constexpr int RT = SB == 16 ? 64 : 32;     // rows per shared-memory tile of the gram / update kernels
-};
+// SB columns per block, a pair rotates PB = 2 SB columns; RT rows per shared-memory tile of the gram / update kernels.
+// Every round streams W and V through HBM once: wider blocks would halve the rounds per sweep, but the PB x PB Gram
+// eigenproblem (PB - 1 dependent Jacobi steps per inner sweep in one CTA) would then dominate every round.
+constexpr int SB = 16, PB = 2 * SB, RT = 64;
 
 // round-robin tournament on nb (even) players: pair p of round r
 __device__ __forceinline__ void rr_pair(int nb, int r, int p, int& i, int& j) {
@@ -36,12 +32,11 @@ __device__ __forceinline__ void rr_pair(int nb, int r, int p, int& i, int& j) {
   else { i = (r + p) % m; j = (r - p + m) % m; }
   if (i > j) { int t = i; i = j; j = t; }
 }
-template <int SB>
 __device__ __forceinline__ int pair_col(int bi, int bj, int c) { return c < SB ? bi * SB + c : bj * SB + (c - SB); }
 
-template <typename T, int SB>
+template <typename T>
 __global__ void __launch_bounds__(256) svd_gram_kernel(const T* __restrict__ W, int64_t R, int nb, int round, T* __restrict__ G, int rsplit) {
-  constexpr int PB = Geo<SB>::PB, RT = Geo<SB>::RT, TPT = PB / 16;   // 16 x 16 threads, TPT x TPT outputs each
+  constexpr int TPT = PB / 16;   // 16 x 16 threads, TPT x TPT outputs each
   __shared__ T tile[PB][RT + 1];
   const int pair = blockIdx.x, chunk = blockIdx.y;
   int bi, bj;
@@ -58,7 +53,7 @@ __global__ void __launch_bounds__(256) svd_gram_kernel(const T* __restrict__ W, 
     for (int idx = threadIdx.x; idx < PB * RT; idx += 256) {
       int c = idx / RT, rr = idx % RT;
       int64_t row = rb + rr;
-      tile[c][rr] = row < r1 ? W[(int64_t)pair_col<SB>(bi, bj, c) * R + row] : zero_<T>();
+      tile[c][rr] = row < r1 ? W[(int64_t)pair_col(bi, bj, c) * R + row] : zero_<T>();
     }
     __syncthreads();
 #pragma unroll 4
@@ -83,9 +78,9 @@ __global__ void __launch_bounds__(256) svd_gram_kernel(const T* __restrict__ W, 
 // Diagonalise the PB x PB Gram matrix of each pair; write the rotation, clear G for the next round,
 // record the largest relative off-diagonal seen BEFORE rotating (sweep convergence measure).
 // Dynamic shared memory: g[PB][PB+1], rm[PB][PB+1] (T), then cs[SB], sn[SB] (double), ph[SB] (T), pp[SB], qq[SB] (int).
-template <typename T, int SB>
+template <typename T>
 __global__ void __launch_bounds__(256) svd_eig_kernel(T* __restrict__ G, T* __restrict__ Rout, unsigned int* conv, double tol_inner, int max_inner) {
-  constexpr int PB = Geo<SB>::PB, LD = PB + 1;
+  constexpr int LD = PB + 1;
   extern __shared__ __align__(16) unsigned char eig_smem[];
   T* g = reinterpret_cast<T*>(eig_smem);
   T* rm = g + PB * LD;
@@ -184,16 +179,15 @@ __global__ void __launch_bounds__(256) svd_eig_kernel(T* __restrict__ G, T* __re
   T* ro = Rout + (int64_t)pair * PB * PB;
   for (int idx = tid; idx < PB * PB; idx += 256) ro[idx] = rm[(idx / PB) * LD + idx % PB];
 }
-template <typename T, int SB>
+template <typename T>
 static size_t eig_smem_bytes() {
-  constexpr int PB = Geo<SB>::PB;
   return 2 * sizeof(T) * PB * (PB + 1) + SB * (2 * sizeof(double) + sizeof(T) + 2 * sizeof(int)) + 16;
 }
 
 // X[:, pair columns] <- X[:, pair columns] * R   (X = W or V; column-contiguous with `rows` rows)
-template <typename T, int SB>
+template <typename T>
 __global__ void __launch_bounds__(256) svd_update_kernel(T* __restrict__ X, int64_t rows, int nb, int round, const T* __restrict__ Rm) {
-  constexpr int PB = Geo<SB>::PB, RT = Geo<SB>::RT, NCG = 256 / RT, CPT = PB / NCG;   // CPT = 8 outputs per thread
+  constexpr int NCG = 256 / RT, CPT = PB / NCG;   // CPT = 8 outputs per thread
   __shared__ T tile[PB][RT];     // read as tile[k][row]: consecutive threads -> consecutive rows (no padding needed)
   __shared__ T rs[PB][PB];       // read as broadcast
   const int pair = blockIdx.x;
@@ -207,7 +201,7 @@ __global__ void __launch_bounds__(256) svd_update_kernel(T* __restrict__ X, int6
     for (int idx = threadIdx.x; idx < PB * RT; idx += 256) {
       int c = idx / RT, r2 = idx % RT;
       int64_t row = rb + r2;
-      tile[c][r2] = row < rows ? X[(int64_t)pair_col<SB>(bi, bj, c) * rows + row] : zero_<T>();
+      tile[c][r2] = row < rows ? X[(int64_t)pair_col(bi, bj, c) * rows + row] : zero_<T>();
     }
     __syncthreads();
     T out[CPT];
@@ -222,7 +216,7 @@ __global__ void __launch_bounds__(256) svd_update_kernel(T* __restrict__ X, int6
     int64_t row = rb + rr;
     if (row < rows) {
 #pragma unroll
-      for (int c = 0; c < CPT; ++c) X[(int64_t)pair_col<SB>(bi, bj, cg * CPT + c) * rows + row] = out[c];
+      for (int c = 0; c < CPT; ++c) X[(int64_t)pair_col(bi, bj, cg * CPT + c) * rows + row] = out[c];
     }
   }
 }
@@ -281,10 +275,9 @@ __global__ void svd_eye_kernel(T* V, int Cp) {
   if (idx < (int64_t)Cp * Cp) V[idx] = (idx / Cp == idx % Cp) ? one_<T>() : zero_<T>();
 }
 
-template <typename T, int SB>
+template <typename T>
 static int svd_real(const tnb200_tensor_t* a, const tnb200_tensor_t* u, const tnb200_tensor_t* s, const tnb200_tensor_t* vh,
                     int32_t* info_dev, cudaStream_t st) {
-  constexpr int PB = Geo<SB>::PB, RT = Geo<SB>::RT;
   const int64_t m = a->shape[0], n = a->shape[1];
   const bool tall = m >= n;
   const int64_t R = tall ? m : n;
@@ -317,22 +310,20 @@ static int svd_real(const tnb200_tensor_t* a, const tnb200_tensor_t* u, const tn
 
   const double eps = 2.220446049250313e-16;
   const double tol = 4.0 * sqrt((double)R) * eps;
-  // inner (Gram) eigen-solver: tolerance / sweep cap (env knobs for experiments; the outer criterion is unchanged)
-  const char* e_tol = getenv("TNB200_SVD_INNER_TOL");
-  const char* e_sw = getenv("TNB200_SVD_INNER_SWEEPS");
-  const double tol_inner = e_tol ? atof(e_tol) : 1e-15;
-  const int max_inner = e_sw ? atoi(e_sw) : 10;
+  // inner (Gram) eigen-solver: tolerance and sweep cap
+  const double tol_inner = 1e-15;
+  const int max_inner = 10;
   int rsplit = (4 * num_sms() + npairs - 1) / npairs;
   int max_split = (int)((R + 4 * RT - 1) / (4 * RT));
   if (rsplit > max_split) rsplit = max_split;
   if (rsplit < 1) rsplit = 1;
   int usplit_w = (int)((R + RT - 1) / RT); if (usplit_w > rsplit * 4) usplit_w = rsplit * 4;
   int usplit_v = (Cp + RT - 1) / RT; if (usplit_v > rsplit * 4) usplit_v = rsplit * 4;
-  const size_t eig_bytes = eig_smem_bytes<T, SB>();
+  const size_t eig_bytes = eig_smem_bytes<T>();
   {
-    static bool attr_done = false;      // per (T, SB) instantiation
+    static bool attr_done = false;      // per T instantiation
     if (!attr_done) {
-      TNB_CHECK_CUDA(cudaFuncSetAttribute(svd_eig_kernel<T, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eig_bytes));
+      TNB_CHECK_CUDA(cudaFuncSetAttribute(svd_eig_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eig_bytes));
       attr_done = true;
     }
   }
@@ -342,10 +333,10 @@ static int svd_real(const tnb200_tensor_t* a, const tnb200_tensor_t* u, const tn
   for (int sw = 0; sw < max_sweeps; ++sw) {
     TNB_CHECK_CUDA(cudaMemsetAsync(conv, 0, sizeof(unsigned int), st));
     for (int r = 0; r < rounds; ++r) {
-      svd_gram_kernel<T, SB><<<dim3(npairs, rsplit), 256, 0, st>>>(W, R, nb, r, G, rsplit);
-      svd_eig_kernel<T, SB><<<npairs, 256, eig_bytes, st>>>(G, Rm, conv, tol_inner, max_inner);
-      svd_update_kernel<T, SB><<<dim3(npairs, usplit_w), 256, 0, st>>>(W, R, nb, r, Rm);
-      svd_update_kernel<T, SB><<<dim3(npairs, usplit_v), 256, 0, st>>>(V, Cp, nb, r, Rm);
+      svd_gram_kernel<T><<<dim3(npairs, rsplit), 256, 0, st>>>(W, R, nb, r, G, rsplit);
+      svd_eig_kernel<T><<<npairs, 256, eig_bytes, st>>>(G, Rm, conv, tol_inner, max_inner);
+      svd_update_kernel<T><<<dim3(npairs, usplit_w), 256, 0, st>>>(W, R, nb, r, Rm);
+      svd_update_kernel<T><<<dim3(npairs, usplit_v), 256, 0, st>>>(V, Cp, nb, r, Rm);
     }
     count_launch(4 * rounds);
     TNB_LAUNCH_CHECK();
@@ -388,6 +379,9 @@ static int svd_real(const tnb200_tensor_t* a, const tnb200_tensor_t* u, const tn
 // no grid-wide barrier inside a sweep, one per sweep for the device-side convergence flag.  No host
 // synchronisation anywhere: the launch is stream-ordered and graph-capturable.
 constexpr int PP_SB = 32, PP_PB = 64, PP_RT = 64, PP_LD = 68, PP_GLD = 65, PP_NST = 4, PP_THREADS = 256;
+// rotation schedule inside a pair: the full 64-column cyclic sweep every 4th round, only the 32 x 32 cross-block pairs in
+// between (numpy model of this kernel, n = 1024: 15 sweeps either way; cross-only in ALL but the first round: 16)
+constexpr int PP_FULL_EVERY = 4;
 
 struct PairParams {
   double* W; int64_t ldw; int ntw;       // W: Cp columns of ldw (= padded rows) doubles; ntw row tiles
@@ -398,7 +392,7 @@ struct PairParams {
   unsigned* conv;                        // [max_sweeps] float bits of the largest relative off-diagonal seen in a sweep
   unsigned* bar;                         // grid barrier counter
   int32_t* info;                         // [0] sweeps, [1] converged
-  int nb, npairs, C, teams, max_sweeps, inner_sweeps, full_every;
+  int nb, npairs, C, teams, max_sweeps;
   float tol;
 };
 
@@ -544,32 +538,30 @@ __global__ void __launch_bounds__(PP_THREADS, 1) svd_pair_kernel(const __grid_co
           }
         }
         __syncthreads();
-        // ---------------- 3. cyclic two-sided Jacobi on G
-        bool rotate = true;
-        for (int isw = 0; isw < p.inner_sweeps; ++isw) {
-          float loc = 0.f;
-          for (int idx = tid; idx < PP_PB * PP_PB; idx += PP_THREADS) {
-            const int i = idx >> 6, j = idx & 63;
-            if (i < j) {
-              const double d = g[i * PP_GLD + i] * g[j * PP_GLD + j];
-              const double x = g[i * PP_GLD + j];
-              if (d > 0.0) loc = fmaxf(loc, (float)(x * x / d));
-            }
+        // ---------------- 3. one cyclic two-sided Jacobi sweep on G, skipped with the update when G is diagonal to tol
+        float loc = 0.f;
+        for (int idx = tid; idx < PP_PB * PP_PB; idx += PP_THREADS) {
+          const int i = idx >> 6, j = idx & 63;
+          if (i < j) {
+            const double d = g[i * PP_GLD + i] * g[j * PP_GLD + j];
+            const double x = g[i * PP_GLD + j];
+            if (d > 0.0) loc = fmaxf(loc, (float)(x * x / d));
           }
-          for (int o = 16; o > 0; o >>= 1) loc = fmaxf(loc, __shfl_xor_sync(0xffffffffu, loc, o));
-          if (lane == 0) red[warp] = loc;
-          __syncthreads();
-          if (tid == 0) {
-            float m = 0.f;
-            for (int w = 0; w < 8; ++w) m = fmaxf(m, red[w]);
-            m = sqrtf(m);
-            s_off = m;
-            if (isw == 0 && member == 0) atomicMax(&p.conv[sweep], __float_as_uint(m));
-          }
-          __syncthreads();
-          if (s_off <= p.tol) { if (isw == 0) rotate = false; break; }
-          // full cyclic schedule (63 steps) every p.full_every-th round, cross-block schedule (32 steps) otherwise
-          const bool cross = p.full_every > 1 && (r % p.full_every) != 0;
+        }
+        for (int o = 16; o > 0; o >>= 1) loc = fmaxf(loc, __shfl_xor_sync(0xffffffffu, loc, o));
+        if (lane == 0) red[warp] = loc;
+        __syncthreads();
+        if (tid == 0) {
+          float m = 0.f;
+          for (int w = 0; w < 8; ++w) m = fmaxf(m, red[w]);
+          m = sqrtf(m);
+          s_off = m;
+          if (member == 0) atomicMax(&p.conv[sweep], __float_as_uint(m));
+        }
+        __syncthreads();
+        if (!(s_off <= p.tol)) {
+          // full cyclic schedule (63 steps) every PP_FULL_EVERY-th round, cross-block schedule (32 steps) otherwise
+          const bool cross = (r % PP_FULL_EVERY) != 0;
           const int nsteps = cross ? PP_SB : PP_PB - 1;
           for (int step = 0; step < nsteps; ++step) {
             if (tid < PP_SB) {
@@ -630,8 +622,6 @@ __global__ void __launch_bounds__(PP_THREADS, 1) svd_pair_kernel(const __grid_co
             }
             __syncthreads();
           }
-        }
-        if (rotate) {
           // ---------------- 4. update: X^T[n][row] = sum_k J^T[n][k] X^T[k][row]; this warp owns 16 output columns n
           for (int idx = tid; idx < PP_PB * PP_PB; idx += PP_THREADS) {
             const int n = idx >> 6, k = idx & 63;
@@ -752,14 +742,6 @@ static int svd_pair_real(const tnb200_tensor_t* a, const tnb200_tensor_t* u, con
   p.gpart = gpart; p.gcount = ctr; p.done = ctr + npairs; p.conv = ctr + npairs + nb; p.bar = ctr + npairs + nb + max_sweeps;
   p.info = info_dev ? info_dev : info;
   p.nb = nb; p.npairs = npairs; p.C = C; p.teams = teams; p.max_sweeps = max_sweeps;
-  const char* e_sw = getenv("TNB200_SVD_INNER_SWEEPS");
-  p.inner_sweeps = e_sw ? atoi(e_sw) : 1;
-  if (p.inner_sweeps < 1) p.inner_sweeps = 1;
-  // rotation schedule inside a pair: the full 64-column cyclic sweep every 4th round, only the 32 x 32 cross-block pairs in
-  // between (numpy model of this kernel, n = 1024: 15 sweeps either way; cross-only in ALL but the first round: 16)
-  const char* e_fe = getenv("TNB200_SVD_FULL_EVERY");
-  p.full_every = e_fe ? atoi(e_fe) : 4;
-  if (p.full_every < 1) p.full_every = 1;
   p.tol = (float)(4.0 * sqrt((double)R) * 2.220446049250313e-16);
   const size_t smem = sizeof(double) * ((size_t)PP_NST * PP_PB * PP_LD + PP_PB * PP_LD + PP_PB * PP_GLD + 2 * PP_SB) + sizeof(int) * 2 * PP_SB + 16;
   static bool attr_done = false;
@@ -808,21 +790,15 @@ __global__ void svd_trunc_kernel(const T* __restrict__ s, int64_t n, int64_t str
 
 using namespace tnb;
 
-// Block width: 16.  The 32-wide variant (half the rounds per sweep, i.e. half the HBM traffic of the gram / update
-// kernels) is kept for real dtypes behind TNB200_SVD_SB=32.  It is not the default: the 64 x 64 Gram eigenproblem
-// (63 dependent Jacobi steps per inner sweep in one CTA) then dominates every round.
 static int svd_dispatch(bool cplx, const tnb200_tensor_t* a, const tnb200_tensor_t* u, const tnb200_tensor_t* s, const tnb200_tensor_t* vh,
                         int32_t* info_dev, cudaStream_t st) {
-  if (cplx) return svd_real<zd, 16>(a, u, s, vh, info_dev, st);
+  if (cplx) return svd_real<zd>(a, u, s, vh, info_dev, st);
   const int64_t cn = a->shape[0] < a->shape[1] ? a->shape[0] : a->shape[1];
-  int sb = 16;
-  const char* algo = getenv("TNB200_SVD_ALGO");       // "rounds" = the launch-per-round kernels below
-  if (cn >= 256 && !(algo && !strcmp(algo, "rounds"))) {
+  if (cn >= 256) {
     set_kernel_name("svd_pair_persistent");
     return svd_pair_real(a, u, s, vh, info_dev, st);
   }
-  if (const char* e = getenv("TNB200_SVD_SB")) { const int v = atoi(e); if (v == 16 || v == 32) sb = v; }
-  return sb == 32 ? svd_real<double, 32>(a, u, s, vh, info_dev, st) : svd_real<double, 16>(a, u, s, vh, info_dev, st);
+  return svd_real<double>(a, u, s, vh, info_dev, st);
 }
 
 extern "C" int32_t tnb200_svd(const tnb200_tensor_t* a, const tnb200_tensor_t* u, const tnb200_tensor_t* s, const tnb200_tensor_t* vh,

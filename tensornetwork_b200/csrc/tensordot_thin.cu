@@ -15,7 +15,6 @@
 //    about the order of k, and a tile's columns can be any 8 columns) so that every thread's loads and
 //    stores are 8/16-byte vectors and every warp instruction covers whole 32-byte sectors.
 #include "common.cuh"
-#include <stdlib.h>
 #include <algorithm>
 #include <vector>
 
@@ -724,9 +723,7 @@ __global__ void __launch_bounds__(256, 1) thin_run_kernel(const __grid_constant_
 }
 
 // ------------------------------------------------------------------------------------------ host side
-static inline int thin_env(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
 static inline unsigned thin_grid_x(int64_t work_items, int64_t batch, int ctas_per_sm) {
-  ctas_per_sm = thin_env("TNB200_THIN_CPS", ctas_per_sm);      // tuning knob (CTAs per SM the grid is sized for)
   int64_t want = ((int64_t)num_sms() * ctas_per_sm + batch - 1) / batch;
   int64_t cap = (work_items + 255) / 256;
   if (want > cap) want = cap;
@@ -773,7 +770,7 @@ template <int DT, int KT, int PT>
 static int launch_mma_kp(int mode, const ThinParams& p, cudaStream_t st) {
   using T = typename DType<DT>::T;
   // registers: ~50 (16x16) .. ~190 (64x64) per thread -> 1..4 CTAs of 256 threads per SM
-  const int ctas = thin_env("TNB200_THIN_MMA_CPS", (KT * PT >= 8) ? 1 : (KT * PT >= 4 ? 2 : 4));
+  const int ctas = (KT * PT >= 8) ? 1 : (KT * PT >= 4 ? 2 : 4);
   int64_t want = ((int64_t)num_sms() * ctas + p.batch - 1) / p.batch;
   const int64_t cap = ((p.L >> 6) + 7) / 8;
   if (want > cap) want = cap;
@@ -799,7 +796,7 @@ static int launch_mma(int mode, const ThinParams& p, cudaStream_t st) {
 
 template <int KT8, int PT>
 static int launch_mma32_kp(int mode, const ThinParams& p, cudaStream_t st) {
-  const int ctas = thin_env("TNB200_THIN_MMA_CPS", (KT8 * PT >= 16) ? 2 : 4);
+  const int ctas = (KT8 * PT >= 16) ? 2 : 4;
   const int64_t nblk = mode == 0 ? (p.L >> 5) : p.L / (16 * (KT8 == 8 ? 2 : 4));
   int64_t want = ((int64_t)num_sms() * ctas + p.batch - 1) / p.batch;
   const int64_t cap = (nblk + 7) / 8;

@@ -51,7 +51,7 @@ def path_to_ssa(n_inputs, path):
   return out
 
 
-def partition_tree(n_inputs, path, step_flops, world, oversub=4, slack=0.03, tensor_bytes=None, small_bytes=1 << 20):
+def partition_tree(n_inputs, path, step_flops, world, oversub=4, slack=0.03):
   """Assign every pairwise step of `path` to a rank.
 
   Returns (owner, transfers, info): owner[s] = rank executing SSA step s (in path order);
@@ -117,10 +117,9 @@ def partition_tree(n_inputs, path, step_flops, world, oversub=4, slack=0.03, ten
     assign_subtree(b, r)
   for t, r in tensor_rank.items():
     assign_subtree(t, r)
-  # steps above the cut: run where the larger-cost operand already lives; steps on small operands all run on `join_rank`
+  # steps above the cut: run where the larger-cost operand already lives
   transfers = []
   where = dict(tensor_rank)
-  join_rank = int(np.argmin(load))
 
   def locate(t):
     if t in where:
@@ -133,13 +132,8 @@ def partition_tree(n_inputs, path, step_flops, world, oversub=4, slack=0.03, ten
       return owner[s]
     a, b, _ = ssa[s]
     ra, rb = locate(a), locate(b)
-    small = tensor_bytes is not None and all(tensor_bytes.get(x, 0) <= small_bytes for x in (a, b) if x >= n_inputs)
     if ra is None and rb is None:
-      r = join_rank if small else int(np.argmin(load))
-    elif small:
-      # both operands are small: gather on ONE rank (a single hop from every producer) instead of a log-depth tree of
-      # hops — the joins above the cut are latency, not bandwidth
-      r = join_rank
+      r = int(np.argmin(load))
     elif ra is None:
       r = rb
     elif rb is None:
@@ -353,10 +347,9 @@ class ShardedNetwork:
   loop) is a binary tree; `partition_tree` cuts it into subtrees packed onto the ranks.  Each rank holds its local
   subtrees as `CompiledNetwork`s (one CUDA-graph replay each) and runs the few steps above the cut eagerly; a subtree
   result consumed on another rank is sent once, point to point (NCCL isend over NVLink) the moment it exists, into a
-  receive the consumer posted before its first contraction.  No collective on the data path."""
+  receive the consumer posted once its own subtrees were enqueued.  No collective on the data path."""
 
-  def __init__(self, backend, shapes, dtype, labels, path, rank, world, group=None, gather_joins=False, early_recv=False,
-               join_graphs=True):
+  def __init__(self, backend, shapes, dtype, labels, path, rank, world, group=None, join_graphs=True):
     from . import drivers  # pylint: disable=import-outside-toplevel
     from . import tensor as T  # pylint: disable=import-outside-toplevel
     self.backend, self.rank, self.world, self.group = backend, rank, world, group
@@ -372,20 +365,9 @@ class ShardedNetwork:
       k = float(np.prod([sizes[l] for l in shared])) if shared else 1.0
       flops.append(2.0 * k * float(np.prod([sizes[l] for l in lab[o]] or [1.0])))
     self.step_flops = flops
-    esz = 8 if T.dtype_code(dtype) in (0, 4, 7) else (16 if T.dtype_code(dtype) == 5 else 4)
-    tensor_bytes = {t: int(np.prod([sizes[l] for l in lab[t]] or [1])) * esz for t in lab}
-    if gather_joins:
-      # Removed: with all small joins on one rank, that rank both receives subtree results from a peer and is sent small
-      # tensors by the same peer in the opposite order; torch's eagerly initialised NCCL group serialises a rank's
-      # point-to-point operations on one stream, so the two ranks wait on each other (observed at 8 GPUs).  A plan whose
-      # point-to-point operations are issued in one global order on every rank would be safe; the tree plan below is (a rank
-      # only sends after it has received everything it needs).
-      raise NotImplementedError("gather_joins deadlocks with serialised NCCL point-to-point operations; use the tree plan")
-    # (gather_joins: every step on small operands on one rank (single hop) instead of the default tree of joins — see above;)
-    # early_recv: receives posted before the first contraction (the NCCL receive kernels then sit on the GPU while it
-    # computes) instead of right before the join; join_graphs: runs of steps above the cut replayed as CUDA graphs
-    self.early_recv, self.join_graphs = early_recv, join_graphs
-    self.owner, self.transfers, self.info = partition_tree(n, path, flops, world, tensor_bytes=tensor_bytes if gather_joins else None)
+    # join_graphs: runs of steps above the cut replayed as CUDA graphs
+    self.join_graphs = join_graphs
+    self.owner, self.transfers, self.info = partition_tree(n, path, flops, world)
     if world > 1 and not schedule_completes(n, ssa, self.owner, self.transfers, world):
       # e.g. 3, 5 or 6 ranks on the benchmark tree: three ranks each start with a large send to the next one.  Every rank
       # reaches the same verdict from the same integers, so all of them raise instead of some of them hanging in NCCL.
@@ -451,15 +433,6 @@ class ShardedNetwork:
     torch = be.torch
     handles, keep = {}, []
     moved = 0
-
-    def post_receives():
-      nonlocal moved
-      for _, t, src in self.incoming:
-        buf = self._recv[t]
-        handles[t] = dist.irecv(buf.t, src, group=self.group)
-        moved += buf.t.numel() * buf.t.element_size()
-    if self.early_recv:
-      post_receives()
     vals = {}
 
     def emit(o, tensor):
@@ -471,9 +444,12 @@ class ShardedNetwork:
         keep.append((buf, dist.isend(buf.t, dst, group=self.group)))
     for root, (_, net) in self.nets.items():
       emit(root, net())
-    if not self.early_recv:
-      post_receives()       # after the local subtrees are enqueued: NCCL orders its stream behind them, the receive
-                            # kernels do not occupy the GPU while it computes
+    # receives are posted after the local subtrees are enqueued: NCCL orders its stream behind them, so the receive
+    # kernels do not occupy the GPU while it computes
+    for _, t, src in self.incoming:
+      buf = self._recv[t]
+      handles[t] = dist.irecv(buf.t, src, group=self.group)
+      moved += buf.t.numel() * buf.t.element_size()
 
     def get(x):
       return self.inputs[x] if x < self.n else vals[x]

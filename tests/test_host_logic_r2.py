@@ -62,11 +62,10 @@ def test_strong_scaling_network_and_partition():
         assert min(send_keys) >= max(recv_keys), (world, r, recv_keys, send_keys)
 
 
-def test_sharded_schedule_has_no_cyclic_wait_with_serialised_p2p():
+def test_sharded_tree_plan_has_no_cyclic_wait_with_serialised_p2p():
   """parallel.schedule_completes: NCCL point-to-point operations that complete strictly in issue order on every rank (torch's
   eagerly initialised process group, large messages).  The tree plan of the benchmark network completes on 2, 4 and 8 ranks;
-  on 3 ranks it would not (ShardedNetwork raises instead of hanging), and neither does the plan that gathers all small joins
-  on one rank — removed after it hung an 8-GPU run."""
+  on 3 ranks it would not (ShardedNetwork raises instead of hanging)."""
   import bench
   from tensornetwork_b200 import drivers, parallel
   from oracle import np_network as nn
@@ -75,19 +74,13 @@ def test_sharded_schedule_has_no_cyclic_wait_with_serialised_p2p():
   flops = [2.0 * m * k * n for m, k, n in nn.network_flops(labels, path, sizes)]
   n = len(labels)
   ssa = parallel.path_to_ssa(n, path)
-  lab = {i: list(l) for i, l in enumerate(labels)}
-  for a, b, o in ssa:
-    sh = [l for l in lab[a] if l in lab[b]]
-    lab[o] = [l for l in lab[a] if l not in sh] + [l for l in lab[b] if l not in sh]
-  tb = {t: int(np.prod([sizes[l] for l in lab[t]] or [1])) * 8 for t in lab}
 
-  def completes(world, tensor_bytes):
-    owner, transfers, _ = parallel.partition_tree(n, path, flops, world, tensor_bytes=tensor_bytes)
+  def completes(world):
+    owner, transfers, _ = parallel.partition_tree(n, path, flops, world)
     return parallel.schedule_completes(n, ssa, owner, transfers, world)
-  ok = {world: completes(world, None) for world in range(2, 9)}
+  ok = {world: completes(world) for world in range(2, 9)}
   assert ok[2] and ok[4] and ok[8], ok           # the world sizes the driver's scaling run uses
   assert not ok[3]                               # three ranks each open with a large send to the next: ShardedNetwork refuses
-  assert not completes(8, tb)                    # the gathered-joins plan: rank 0 and rank 1 wait on each other
 
 
 def test_blocksparse_degeneracy_arithmetic():
