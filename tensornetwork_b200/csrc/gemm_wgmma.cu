@@ -55,6 +55,34 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
 }
+// The same load issued to both CTAs of a 2-CTA cluster (mask 0b11): the box lands at the same shared-memory offset in
+// each and signals the mbarrier at the same offset in each.
+__device__ __forceinline__ void tma_load_5d_pair(uint32_t dst, const CUtensorMap* map, uint32_t bar,
+                                                 int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2], %8;"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "h"((uint16_t)0x3) : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// Arrive on the mbarrier at the same shared-memory offset as `bar` in CTA `cta` of the cluster.  Default semantics
+// (release at CTA scope): the arrive only has to follow the wgmma reads of the slot, which wgmma.wait_group has
+// retired.  .release.cluster puts a MEMBAR.ALL.GPU before every arrive: the chain's k loop took 1.6x as long with
+// it in one measurement (bench cfg2, H100 SXM, 400 W).
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}"
+      ::"r"(bar), "r"(cta) : "memory");
+}
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
                ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2) : "memory");
@@ -108,16 +136,38 @@ constexpr int kThreads = 384;
 // (intermediates are produced and consumed while still in L2), and inter-step dependencies are tracked per
 // (step, sample) with release/acquire counters in global memory: once the TMA stores of an output tile have
 // completed, the CTA's store warp publishes the tile with red.release, the TMA producer of a dependent tile spins
-// with ld.acquire + fence.proxy.async before its first load.  Tiles are assigned to CTAs round-robin in sequence
-// order and all CTAs are co-resident (grid <= resident CTAs), so a tile only ever waits for tiles that are earlier
-// in the sequence: no deadlock.
+// with ld.acquire + fence.proxy.async before its first load.
+//
+// The unit of the sequence is a *pair* of tiles: the same step, sample and N tile, M tiles 2j and 2j + 1, run by
+// the two CTAs of a 2-CTA cluster (rank r takes M tile 2j + r).  The pair shares its B tile: each CTA loads its own
+// A tile and one half of B, multicast into both CTAs, so a pair reads 2 x 128 + 256 operand rows per k block instead
+// of 2 x (128 + 256), a third less L2 -> SM traffic (a 128 x 256 tile alone reads 85 flop per operand byte).  A
+// ring slot is refilled only when the consumers of BOTH CTAs have released it: the empty barrier counts the
+// consumer warps of the pair, each of which arrives in its own CTA and in the partner.  Both
+// producers of a pair wait on the same dependency counters and walk the ring in the same order, which keeps the two
+// CTAs in step.  When tiles_m is odd the partner of the last M tile has no tile: it still loads and multicasts its
+// half of B and releases its slots, but issues no MMAs and stores and publishes nothing.  Each CTA publishes its own
+// tile, so the counters still count tiles.  Pairs are assigned to clusters round-robin in sequence order and all
+// clusters are co-resident (grid <= resident clusters), so a pair only ever waits for pairs that are earlier in the
+// sequence: no deadlock.
 //
 // The chain's epilogue overlaps the next tile's k loop: the consumers convert the accumulators into a shared-memory
 // staging buffer (128-byte swizzled 64-row x 128-byte boxes: conflict-free stores) and go on to the next tile; warp
 // 1 writes the buffer out with TMA stores through a per-step tensor map of C, frees it once the TMA engine has
-// read it, and publishes the tile once the stores are complete.  16-bit chains run 128 x 256 tiles (3 ring stages
-// of 48 KB + 64 KB staging), tf32 chains 128 x 128 (their MN-major transpose slot doubles a stage, so their 32 KB
-// tile half is staged in two 16 KB passes to keep 3 stages of 64 KB).
+// read it, and publishes the tile once the stores are complete.  16-bit chains run 128 x 256 tiles, tf32 chains
+// 128 x 128 (their MN-major transpose slot doubles a stage).  Either way a consumer warpgroup's 32 KB half of the
+// output tile is staged in two 16 KB passes, so that the ring gets 4 stages of 48 KB (16-bit) or 3 of 64 KB (tf32).
+//
+// Measured on the bench's cfg2 chain (H100 SXM, 700 W; tools/chain_phases.py, one run per build): the 16-bit k loop
+// waits on load latency more than on L2 bandwidth.  A stage is about 0.55 us of MMAs at 128 x 256.
+//   3 stages, no pairs: launch 7.22 ms, consumers' wait for a stage 3.56 ms per CTA
+//   pairs, 3 stages:    launch 7.19 ms, wait 3.57 ms (a run of its own against 7.16 / 3.58 ms without pairs)
+//   4 stages, no pairs: launch 6.58 ms, wait 1.99 ms
+//   pairs, 4 stages:    launch 6.85 ms, wait 1.93 ms
+// So the 4th stage (room made by the two-pass epilogue) is what shortens the wait.  A third less L2 traffic does
+// not, and a refill that waits for the slower CTA of the pair costs launch time.  Over three alternated bench runs
+// the step took 10.28-10.45 ms (3 stages, no pairs), 9.96-10.08 ms (4 stages, no pairs) and 10.01-10.12 ms (pairs,
+// 4 stages).
 struct alignas(64) ChainStepDev {
   CUtensorMap tmA, tmB, tmC;
   TcParams p;
@@ -125,19 +175,19 @@ struct alignas(64) ChainStepDev {
   uint32_t need_a, need_b;        // counter value of that step's (sample) entry when it is complete: its tiles
   int tiles_per_sample;
 };
-struct ChainSeg { long long tile0; int step, sample0, nsamples, pad; };
+struct ChainSeg { long long tile0; int step, sample0, nsamples, pad; };   // tile0: first pair of the segment
 struct ChainParams {
   const ChainStepDev* steps;
   const ChainSeg* segs;
   uint32_t* done;                 // [nsteps][batch] completion counters (zeroed before every launch)
-  long long num_tiles;
+  long long num_tiles;            // pairs
   int nsegs, batch, stages, stage_bytes;
 };
 constexpr int kConsumerWarps = 8;     // consumer warps per CTA: each releases ring slots
-// Chain epilogue staging, per consumer warpgroup (64 rows x 512 bytes of output = four 8 KB boxes).
+// Chain epilogue staging, per consumer warpgroup: 64 rows x 512 bytes of output = four 8 KB boxes, two per pass.
 constexpr int kChainBN16 = 256, kChainBN32 = 128;
 constexpr int kBoxBytes = 64 * 128;
-constexpr int chain_stage_half(int kind) { return kind == 2 ? 2 * kBoxBytes : 4 * kBoxBytes; }
+constexpr int kChainStageHalf = 2 * kBoxBytes;
 
 // Everything one launch needs: a single GEMM (tile params + maps) or a chain.
 struct KernelArgs {
@@ -187,9 +237,11 @@ struct Tile {
   const CUtensorMap *ma, *mb;
   const ChainStepDev* sd;         // chain step (nullptr for a single GEMM)
   int bi, mi, ni, step;
+  bool live;                      // false: the partner of the last M tile when tiles_m is odd (chain only)
 };
+// Single GEMM: `tile` is a tile.  Chain: `tile` is a pair and `rank` the CTA's rank in the cluster.
 template <bool CHAIN>
-__device__ __forceinline__ void decode_tile(const KernelArgs& a, long long tile, int& cursor, Tile& t) {
+__device__ __forceinline__ void decode_tile(const KernelArgs& a, long long tile, int rank, int& cursor, Tile& t) {
   if (!CHAIN) {
     uint32_t x = (uint32_t)tile;
     const uint32_t tn = (uint32_t)a.p.tiles_n, tm = (uint32_t)a.p.tiles_m;
@@ -197,18 +249,20 @@ __device__ __forceinline__ void decode_tile(const KernelArgs& a, long long tile,
     t.mi = (int)(x % tm);
     t.bi = (int)(x / tm);
     t.p = &a.p; t.ma = &a.tmA; t.mb = &a.tmB; t.sd = nullptr; t.step = 0;
+    t.live = true;
   } else {
     const ChainParams& cp = a.cp;
     while (cursor + 1 < cp.nsegs && tile >= cp.segs[cursor + 1].tile0) ++cursor;
     const ChainSeg sg = cp.segs[cursor];
     const ChainStepDev* sd = cp.steps + sg.step;
     uint32_t local = (uint32_t)(tile - sg.tile0);
-    const uint32_t tn = (uint32_t)sd->p.tiles_n, tm = (uint32_t)sd->p.tiles_m;
+    const uint32_t tn = (uint32_t)sd->p.tiles_n, tm = (uint32_t)sd->p.tiles_m, pm = (tm + 1) / 2;
     t.ni = (int)(local % tn); local /= tn;
-    t.mi = (int)(local % tm);
-    t.bi = sg.sample0 + (int)(local / tm);
+    t.mi = 2 * (int)(local % pm) + rank;
+    t.bi = sg.sample0 + (int)(local / pm);
     t.step = sg.step;
     t.p = &sd->p; t.ma = &sd->tmA; t.mb = &sd->tmB; t.sd = sd;
+    t.live = (uint32_t)t.mi < tm;
   }
 }
 
@@ -256,10 +310,30 @@ __device__ __forceinline__ void mma_k(float* d, uint64_t a, uint64_t b, uint32_t
   }
 }
 
+// Release ring slot `bar` (its empty barrier) from one consumer warp: in the chain, to the producers of both CTAs of
+// the pair, since either may refill the slot's B half in both.
+template <bool PAIR>
+__device__ __forceinline__ void release_slot(uint32_t bar) {
+  if constexpr (PAIR) { mbar_arrive_cluster(bar, 0); mbar_arrive_cluster(bar, 1); }
+  else mbar_arrive(bar);
+}
+
+// The k loop of the partner that has no tile: it takes every stage as the live CTA does (so that the partner's
+// multicast has landed before the slot is released) and releases it at once.
+__device__ __forceinline__ void drainloop(int S, uint32_t bar_base, int num_kb, int lane, int& s, uint32_t& ph) {
+#pragma unroll 1
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(bar_base + 8u * s, ph);
+    __syncwarp();
+    if (lane == 0) release_slot<true>(bar_base + 8u * (S + s));
+    if (++s == S) { s = 0; ph ^= 1; }
+  }
+}
+
 // The k loop of one tile for one consumer warpgroup.  The operand majorness is a template parameter so that
 // the wgmma sequence is straight-line code.  Descriptor fields: a K-major operand advances 32 bytes per MMA,
 // an MN-major one 16 K rows (2 KB); MN chunks of 64 elements are BK rows x 128 B apart.
-template <int KIND, int BN, int TA, int TB>
+template <int KIND, int BN, int TA, int TB, bool PAIR>
 __device__ __forceinline__ void mainloop(float* d, uint8_t* smem, int stage_bytes, int S, uint32_t bar_base, int num_kb,
                                          int a_mn, int b_mn, int wg, int ctid, int lane, int& s, uint32_t& ph) {
   constexpr int BK = kRowBytes / (KIND == 2 ? 4 : 2);
@@ -286,14 +360,14 @@ __device__ __forceinline__ void mainloop(float* d, uint8_t* smem, int stage_byte
     if (prev >= 0) {
       wg_wait<1>();                                            // the MMAs of the previous stage have retired
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar_base + 8u * (S + prev));
+      if (lane == 0) release_slot<PAIR>(bar_base + 8u * (S + prev));
     }
     prev = s;
     if (++s == S) { s = 0; ph ^= 1; }
   }
   wg_wait<0>();
   __syncwarp();
-  if (lane == 0) mbar_arrive(bar_base + 8u * (S + prev));
+  if (lane == 0) release_slot<PAIR>(bar_base + 8u * (S + prev));
 }
 
 __device__ __forceinline__ void store_one(const TcParams& p, int64_t off, float v) {
@@ -321,7 +395,7 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
   const int S = CHAIN ? args.cp.stages : args.p.stages;
   const long long num_tiles = CHAIN ? args.cp.num_tiles : args.p.num_tiles;
   // chain: the epilogue staging buffer (one half per consumer warpgroup) follows the ring
-  constexpr int STAGE_HALF = chain_stage_half(KIND);
+  constexpr int STAGE_HALF = kChainStageHalf;
   const uint32_t staging = smem_u32(smem + (size_t)S * STAGE_BYTES);
   uint64_t* bars = (uint64_t*)(smem + (size_t)S * STAGE_BYTES + (CHAIN ? 2 * STAGE_HALF : 0));
   const uint32_t bar_base = smem_u32(bars);
@@ -337,38 +411,50 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&args.tmA) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&args.tmB) : "memory");
     }
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
+    // chain: the consumer warps of both CTAs of the pair release a slot
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), (CHAIN ? 2 : 1) * kConsumerWarps);
+    }
     if (CHAIN)
       for (int wg = 0; wg < 2; ++wg) { mbar_init(staged_bar(wg), 4); mbar_init(freed_bar(wg), 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
-  const long long first = blockIdx.x, step = gridDim.x;
+  // chain: the partner's multicast loads and remote arrives target this CTA's barriers from the start
+  if constexpr (CHAIN) cluster_sync();
+  else __syncthreads();
+  // chain: cluster c runs pairs c, c + clusters, ...; its CTA of rank r takes M tile 2j + r of each
+  const int rank = CHAIN ? (int)cluster_ctarank() : 0;
+  const long long first = CHAIN ? blockIdx.x / 2 : blockIdx.x, step = CHAIN ? gridDim.x / 2 : gridDim.x;
 
   if (warp == 0) {
     // ===================================================== TMA producer (whole warp)
-    // lane l owns "load slot" l of a stage: one 128-byte-wide box of A (slots 0..nA-1) or of B (nA..nA+nB-1),
-    // so the boxes of a stage are issued in parallel; inside the k loop a lane only advances its contracted-mode
-    // coordinates incrementally.
+    // lane l owns "load slot" l of a stage: one box of A (slots 0..nA-1) or of B (nA..nA+nB-1), so the boxes of a
+    // stage are issued in parallel; inside the k loop a lane only advances its contracted-mode coordinates
+    // incrementally.  A box covers 128 bytes of an MN-major operand's free mode, or all kBM rows of a K-major A and
+    // BN / B_SPLIT rows of a K-major B.  In the chain each CTA loads B half `rank` and multicasts it to the pair.
+    constexpr int B_SPLIT = CHAIN ? 2 : 1;
     int s = 0; uint32_t ph = 0;
     int cursor = 0;
     for (long long tile = first; tile < num_tiles; tile += step) {
       Tile t;
-      decode_tile<CHAIN>(args, tile, cursor, t);
+      decode_tile<CHAIN>(args, tile, rank, cursor, t);
       const TcParams& p = *t.p;
       const int a_mn = p.a_mn, b_mn = p.b_mn;
-      const int nA = a_mn ? kBM / CHUNK : 1;
-      const int nB = b_mn ? BN / CHUNK : 1;
+      const int nA = t.live ? (a_mn ? kBM / CHUNK : 1) : 0;
+      const int nB = b_mn ? BN / CHUNK / B_SPLIT : 1;
       const bool mine = lane < nA + nB;
       const bool is_a = lane < nA;
-      const int c = is_a ? lane : lane - nA;                       // chunk index inside the operand tile
       const bool mn = is_a ? (a_mn != 0) : (b_mn != 0);
+      const int c = is_a ? lane : rank * nB + lane - nA;          // box index inside the operand tile
+      const int fbox = mn ? CHUNK : (is_a ? kBM : BN / B_SPLIT);  // free elements of one box (BK = CHUNK K rows)
       const uint32_t fe = is_a ? p.a_fe : p.b_fe, ke = is_a ? p.a_ke : p.b_ke;
       const CUtensorMap* map = is_a ? t.ma : t.mb;
-      uint32_t dst_off = (is_a ? 0u : (uint32_t)A_BYTES) + (mn ? (uint32_t)c * (BK * kRowBytes) : 0u);
+      uint32_t dst_off = (is_a ? 0u : (uint32_t)A_BYTES) + (uint32_t)(c * fbox * kRowBytes);
       if (KIND == 2 && mn) dst_off += A_BYTES + B_BYTES;          // f32 MN-major: staging slot, transposed by the consumers
-      const int f = is_a ? t.mi * kBM + (mn ? c * CHUNK : 0) : t.ni * BN + (mn ? c * CHUNK : 0);
+      const int f = (is_a ? t.mi * kBM : t.ni * BN) + c * fbox;
       const int f_in = fe ? (int)((uint32_t)f % fe) : f, f_out = fe ? (int)((uint32_t)f / fe) : 0;
+      const uint32_t tx_bytes = (t.live ? A_BYTES : 0) + B_BYTES;  // B: both halves land here
       const int num_kb = p.num_kb;
       if (CHAIN) {
         // operands produced by earlier steps of this launch: wait until every tile of (that step, this sample) is out
@@ -386,12 +472,13 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(empty_bar(s), ph ^ 1);                          // slot free (every lane observes it)
         const uint32_t full = full_bar(s);
-        if (lane == 0) mbar_expect_tx(full, (uint32_t)(A_BYTES + B_BYTES));
+        if (lane == 0) mbar_expect_tx(full, tx_bytes);
         __syncwarp();
         if (mine) {
           const uint32_t dst = smem_u32(smem + (size_t)s * STAGE_BYTES) + dst_off;
-          if (!mn) tma_load_5d(dst, map, full, k_in, f_in, f_out, k_out, t.bi);
-          else     tma_load_5d(dst, map, full, f_in, k_in, k_out, f_out, t.bi);
+          const int x0 = mn ? f_in : k_in, x1 = mn ? k_in : f_in, x2 = mn ? k_out : f_out, x3 = mn ? f_out : k_out;
+          if (CHAIN && !is_a) tma_load_5d_pair(dst, map, full, x0, x1, x2, x3, t.bi);
+          else                tma_load_5d(dst, map, full, x0, x1, x2, x3, t.bi);
         }
         k_in += BK;
         if (ke && (uint32_t)k_in >= ke) { k_in = 0; ++k_out; }
@@ -409,17 +496,21 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
     float d[BN / 2];
     for (long long tile = first; tile < num_tiles; tile += step) {
       Tile t;
-      decode_tile<CHAIN>(args, tile, cursor, t);
+      decode_tile<CHAIN>(args, tile, rank, cursor, t);
       const TcParams& p = *t.p;
       const int a_mn = p.a_mn, b_mn = p.b_mn, num_kb = p.num_kb;
+      if (CHAIN && !t.live) {
+        drainloop(S, bar_base, num_kb, lane, s, ph);
+        continue;
+      }
       TNB_PHASE(const unsigned long long tk = phase_clock();)
       if constexpr (KIND == 2) {
-        mainloop<KIND, BN, 0, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        mainloop<KIND, BN, 0, 0, CHAIN>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
       } else {
-        if (a_mn && b_mn) mainloop<KIND, BN, 1, 1>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
-        else if (a_mn) mainloop<KIND, BN, 1, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
-        else if (b_mn) mainloop<KIND, BN, 0, 1>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
-        else mainloop<KIND, BN, 0, 0>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        if (a_mn && b_mn) mainloop<KIND, BN, 1, 1, CHAIN>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        else if (a_mn) mainloop<KIND, BN, 1, 0, CHAIN>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        else if (b_mn) mainloop<KIND, BN, 0, 1, CHAIN>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
+        else mainloop<KIND, BN, 0, 0, CHAIN>(d, smem, STAGE_BYTES, S, bar_base, num_kb, a_mn, b_mn, wg, ctid, lane, s, ph);
       }
       TNB_PHASE(const unsigned long long te = phase_clock(); if (ctid == 0) TNB_PHASE_ADD(2, te - tk);)
       const int r0 = (wt >> 5) * 16 + (lane >> 2);
@@ -493,7 +584,8 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
     uint32_t sph = 0;
     for (long long tile = first; tile < num_tiles; tile += step) {
       Tile t;
-      decode_tile<CHAIN>(args, tile, cursor, t);
+      decode_tile<CHAIN>(args, tile, rank, cursor, t);
+      if (!t.live) continue;
       const CUtensorMap* mc = &t.sd->tmC;
 #pragma unroll 1
       for (int pass = 0; pass < 4 * kBoxBytes / STAGE_HALF; ++pass) {
@@ -520,6 +612,8 @@ gemm_wgmma_kernel(const __grid_constant__ KernelArgs args) {
       red_release_add_u32(args.cp.done + (size_t)t.step * args.cp.batch + t.bi, 1u);
     }
   }
+  // chain: neither CTA exits while its partner can still arrive on its barriers
+  if constexpr (CHAIN) cluster_sync();
 }
 
 // ------------------------------------------------------------------------------- host side
@@ -703,7 +797,8 @@ static int tc_prepare(const GemmProblem& g, bool chain_mode, TcPrep& o) {
   bool a_mn = false, b_mn = false;
   int rc = encode_operand(&o.tmA, g.dtype, g.A, g.M, g.K, g.batch, kBM, a_mn, p.a_fe, p.a_ke);
   if (rc) return rc;
-  rc = encode_operand(&o.tmB, g.dtype, g.B, g.N, g.K, g.batch, BN, b_mn, p.b_fe, p.b_ke);
+  // chain: each CTA of a pair loads half of the B tile (a K-major box of BN / 2 rows)
+  rc = encode_operand(&o.tmB, g.dtype, g.B, g.N, g.K, g.batch, chain_mode ? BN / 2 : BN, b_mn, p.b_fe, p.b_ke);
   if (rc) return rc;
   p.a_mn = a_mn; p.b_mn = b_mn;
   o.stage_bytes = stage_bytes_of(g.dtype, BN, a_mn, b_mn);
@@ -785,6 +880,21 @@ struct ChainHandle {
   unsigned grid = 0;
 };
 
+// Launch configuration of the chained kernel: 2-CTA clusters along x (the pairs).
+struct PairLaunch {
+  cudaLaunchAttribute attr;
+  cudaLaunchConfig_t cfg;
+  PairLaunch(unsigned grid, size_t smem, cudaStream_t st) {
+    memset(&attr, 0, sizeof(attr));
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+  }
+  PairLaunch(const PairLaunch&) = delete;
+};
+
 int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, const int* dep_b, int* first_unsupported,
                       void** handle) {
   *handle = nullptr;
@@ -838,25 +948,33 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
     }
   }
   // the ring gets what the 227 KB of shared memory leave beside the epilogue staging and the barriers
-  const int staging = 2 * chain_stage_half(kind);
+  const int staging = 2 * kChainStageHalf;
   int stages = (227 * 1024 - 1024 - staging - 256) / max_stage;
   if (stages > 8) stages = 8;
   if (stages < 2) return TNB200_ERR_UNSUPPORTED;
   const size_t smem = smem_of(stages, max_stage) + staging + 4 * 8;
-  // every CTA of the launch must be resident (tiles wait on earlier tiles): ask the runtime how many fit
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)fn, kThreads, smem) != cudaSuccess) { cudaGetLastError(); per_sm = 0; }
-  const int ctas = per_sm * num_sms();
-  if (ctas < 1) return TNB200_ERR_UNSUPPORTED;
-  // ---- tile sequence.  The batch is cut into rounds of about G samples and every round is carried through ALL
+  // every cluster of the launch must be resident (pairs wait on earlier pairs): ask the runtime how many fit
+  int clusters = 0;
+  {
+    PairLaunch pl(2 * num_sms(), smem, nullptr);
+    if (cudaOccupancyMaxActiveClusters(&clusters, (void*)fn, &pl.cfg) != cudaSuccess) {
+      cudaGetLastError();
+      clusters = 0;
+    }
+  }
+  if (clusters < 1) return TNB200_ERR_UNSUPPORTED;
+  // pairs per sample of each step: N tiles x M tile pairs
+  std::vector<int> pps(nsteps);
+  for (int i = 0; i < nsteps; ++i) pps[i] = (int)(steps[i].p.tiles_n * ((steps[i].p.tiles_m + 1) / 2));
+  // ---- pair sequence.  The batch is cut into rounds of about G samples and every round is carried through ALL
   // steps before the next one starts, so a step's results are consumed soon after they are produced.  A round
-  // must be wide enough that a dependent tile is at least one full wave of tiles behind its producers, and should
+  // must be wide enough that a dependent pair is at least one full wave of pairs behind its producers, and should
   // be as wide as the L2 allows: the operands and results of one step of the round then stay in L2 for the next.
   auto env_int = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
-  int min_tps = steps[0].tiles_per_sample;
-  for (int i = 1; i < nsteps; ++i) if (steps[i].tiles_per_sample < min_tps) min_tps = steps[i].tiles_per_sample;
-  if (batch * min_tps < ctas && !env_int("TNB200_CHAIN_FORCE", 0))
-    return TNB200_ERR_UNSUPPORTED;      // too few tiles per step to hide the producer->consumer latency: launch step by step
+  int min_pps = pps[0];
+  for (int i = 1; i < nsteps; ++i) if (pps[i] < min_pps) min_pps = pps[i];
+  if (batch * min_pps < clusters && !env_int("TNB200_CHAIN_FORCE", 0))
+    return TNB200_ERR_UNSUPPORTED;  // too few pairs per step to hide the producer->consumer latency: go step by step
   int l2 = 0;
   {
     int dev = 0;
@@ -865,7 +983,7 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
       l2 = 0;
     }
   }
-  const int g_wave = (ctas + min_tps - 1) / min_tps;
+  const int g_wave = (clusters + min_pps - 1) / min_pps;
   const int g_l2 = (int)(l2 / sample_bytes);
   int G = env_int("TNB200_CHAIN_G", g_wave > g_l2 ? g_wave : g_l2);
   if (G < 1) G = 1;
@@ -879,7 +997,7 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
       ChainSeg sg;
       sg.tile0 = tile0; sg.step = i; sg.sample0 = (int)r0; sg.nsamples = (int)(r1 - r0); sg.pad = 0;
       segs.push_back(sg);
-      tile0 += (long long)(r1 - r0) * steps[i].tiles_per_sample;
+      tile0 += (long long)(r1 - r0) * pps[i];
     }
   }
   ChainHandle* h = new ChainHandle();
@@ -904,7 +1022,7 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
   cp.stages = stages; cp.stage_bytes = max_stage;
   h->args.stage_bytes = max_stage;
   h->smem = smem;
-  h->grid = (unsigned)(tile0 < ctas ? tile0 : ctas);
+  h->grid = (unsigned)(2 * (tile0 < clusters ? tile0 : clusters));
   *handle = h;
   return 0;
 }
@@ -913,8 +1031,8 @@ int gemm_chain_launch(void* handle, cudaStream_t st) {
   ChainHandle* h = (ChainHandle*)handle;
   if (!h) return TNB200_ERR_INVALID;
   TNB_CHECK_CUDA(cudaMemsetAsync(h->d_done, 0, h->done_bytes, st));
-  kernel_of(h->kind, 0, true)<<<h->grid, kThreads, h->smem, st>>>(h->args);
-  TNB_LAUNCH_CHECK();
+  PairLaunch pl(h->grid, h->smem, st);
+  TNB_CHECK_CUDA(cudaLaunchKernelEx(&pl.cfg, kernel_of(h->kind, 0, true), h->args));
   count_launch();
   set_kernel_name(h->kind == 2 ? "wgmma_chain_tf32" : "wgmma_chain_16");
   return 0;

@@ -8,7 +8,9 @@ averaged over CTAs, the %globaltimer time spent in:
   full_wait    the consumers waiting for a ring stage (starved of operands; measured on one consumer thread)
   k_loop       the whole k loop, full_wait included
   epilogue     from the end of the k loop to the point the tile needs nothing more from the consumers
-and, for --G values, the same for other round sizes (TNB200_CHAIN_G).
+and, for --G values, the same for other round sizes (TNB200_CHAIN_G).  It also prints the chain's L2 -> SM operand
+feed per launch and its rate over the launch time: the operand bytes the kernel's tiles read, computed from the shapes
+(per pair of M tiles: two 128-row A tiles and one shared B tile of BN rows, each K elements deep), not a counter.
 
   python tools/chain_phases.py [--G 9 17 19 38] [--reps 20] [--networks 74]
 """
@@ -25,6 +27,15 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 PHASES = ["chain_wait", "full_wait", "k_loop", "epilogue", "cta_life", "tiles"]
+BM, BN_16, BN_32 = 128, 256, 128        # the chained kernel's tile (16-bit operands / tf32)
+
+
+def feed_bytes(m, k, n, esize):
+  """L2 -> SM operand bytes of one sample of one chain step (M x K times K x N, `esize`-byte operands): per N tile and
+  pair of M tiles, the pair's A tiles (one when tiles_m is odd and the pair is the last) and one shared B tile"""
+  bn = BN_32 if esize == 4 else BN_16
+  tm, tn = -(-m // BM), -(-n // bn)
+  return tn * (tm * BM + -(-tm // 2) * bn) * k * esize
 
 
 def build_phase_lib(out_dir):
@@ -81,6 +92,7 @@ def main():
     t = be.randn(shapes[i], np.float32, seed=1 + i)
     t *= 1.0 / np.sqrt(dims[i] * d)
     kets.append(be.astype(t, "bfloat16"))
+  esize = kets[0].t.element_size()
   props = torch.cuda.get_device_properties(0)
   print("device %s, %d SMs, L2 %.0f MB" % (props.name, props.multi_processor_count, props.L2_cache_size / 2**20))
   for G in [None] + list(args.G):
@@ -95,6 +107,7 @@ def main():
     ch = max(net.chains, key=lambda c: len(c.steps))
     pairwise = [i for i, st in enumerate(net.steps) if st[0] != "transpose"]     # `work` skips transposes
     flops = NB * sum(2.0 * np.prod(work[pairwise.index(s)]) for s in ch.steps)
+    feed = NB * sum(feed_bytes(*work[pairwise.index(s)], esize) for s in ch.steps)
     for _ in range(3):
       ch.launch()
     torch.cuda.synchronize()
@@ -109,9 +122,10 @@ def main():
     ph = read(True)
     ctas = int(np.count_nonzero(ph[:, 5]))
     per = ph[:ctas].mean(axis=0) / args.reps
-    print("G=%-8s chain %d steps: %8.1f us/launch  %6.1f TFLOP/s  | per CTA, us/launch: %s  tiles %.1f" % (
-        "default" if G is None else G, len(ch.steps), us, flops / us / 1e6,
-        "  ".join("%s %.1f" % (n, per[i] / 1e3) for i, n in enumerate(PHASES[:5])), per[5]), flush=True)
+    print("G=%-8s chain %d steps: %8.1f us/launch  %6.1f TFLOP/s  feed %.2f GB %.2f TB/s  | per CTA, us/launch: %s  "
+          "tiles %.1f  (%d CTAs)" % (
+              "default" if G is None else G, len(ch.steps), us, flops / us / 1e6, feed / 1e9, feed / us / 1e6,
+              "  ".join("%s %.1f" % (n, per[i] / 1e3) for i, n in enumerate(PHASES[:5])), per[5], ctas), flush=True)
     del net, ch
 
 
