@@ -912,7 +912,7 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
   const int64_t batch = probs[0].batch;
   std::vector<ChainStepDev> steps(nsteps);
   int max_stage = 0;
-  int64_t sample_bytes = 0;       // largest per-sample footprint of one step: both operands and the result
+  std::vector<int64_t> step_bytes(nsteps), out_bytes(nsteps);   // per sample: operands + result, result
   for (int i = 0; i < nsteps; ++i) {
     const GemmProblem& g = probs[i];
     if (g.conjA || g.conjB || g.swapped) return reject(i, TNB200_ERR_UNSUPPORTED);
@@ -930,8 +930,8 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
     sd.dep_a = dep_a[i]; sd.dep_b = dep_b[i];
     sd.tiles_per_sample = (int)(prep.p.tiles_m * prep.p.tiles_n);
     if (prep.stage_bytes > max_stage) max_stage = prep.stage_bytes;
-    const int64_t b = (g.M * g.K + g.N * g.K + g.M * g.N) * es_of(dtype);
-    if (b > sample_bytes) sample_bytes = b;
+    step_bytes[i] = (g.M * g.K + g.N * g.K + g.M * g.N) * es_of(dtype);
+    out_bytes[i] = g.M * g.N * es_of(dtype);
   }
   for (int i = 0; i < nsteps; ++i) {
     if (steps[i].dep_a >= 0) steps[i].need_a = (uint32_t)steps[steps[i].dep_a].tiles_per_sample;
@@ -967,9 +967,13 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
   std::vector<int> pps(nsteps);
   for (int i = 0; i < nsteps; ++i) pps[i] = (int)(steps[i].p.tiles_n * ((steps[i].p.tiles_m + 1) / 2));
   // ---- pair sequence.  The batch is cut into rounds of about G samples and every round is carried through ALL
-  // steps before the next one starts, so a step's results are consumed soon after they are produced.  A round
-  // must be wide enough that a dependent pair is at least one full wave of pairs behind its producers, and should
-  // be as wide as the L2 allows: the operands and results of one step of the round then stay in L2 for the next.
+  // steps, in step order, before the next one starts, so a step's results are consumed soon after they are produced.
+  // G follows from the dependencies.  A round must be wide enough that the segment of a step starts at least one
+  // full wave of pairs after the segment of each step it reads: in a run that is the segment just before it, in a
+  // group of independent runs (the heads of the four MPS ramps) it lies several segments back.  And a round should
+  // be as wide as the L2 allows: per sample it keeps live the results that a later step of the round has yet to read,
+  // besides the operands and result of the step that runs.  In a run the only such result is the running step's
+  // operand, so the bound is the largest step alone.
   auto env_int = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
   int min_pps = pps[0];
   for (int i = 1; i < nsteps; ++i) if (pps[i] < min_pps) min_pps = pps[i];
@@ -983,8 +987,26 @@ int gemm_chain_create(int nsteps, const GemmProblem* probs, const int* dep_a, co
       l2 = 0;
     }
   }
-  const int g_wave = (clusters + min_pps - 1) / min_pps;
-  const int g_l2 = (int)(l2 / sample_bytes);
+  int g_wave = 1;
+  std::vector<int> last_reader(nsteps, -1);
+  for (int i = 0; i < nsteps; ++i) {
+    for (const int d : {dep_a[i], dep_b[i]}) {
+      if (d < 0) continue;
+      last_reader[d] = i;
+      int64_t gap = 0;                // pairs per sample from the start of step d's segment to the start of step i's
+      for (int j = d; j < i; ++j) gap += pps[j];
+      const int g = (int)((clusters + gap - 1) / gap);
+      if (g > g_wave) g_wave = g;
+    }
+  }
+  int64_t live_bytes = 0;
+  for (int i = 0; i < nsteps; ++i) {
+    int64_t live = step_bytes[i];
+    for (int j = 0; j < i; ++j)
+      if (last_reader[j] > i && dep_a[i] != j && dep_b[i] != j) live += out_bytes[j];
+    if (live > live_bytes) live_bytes = live;
+  }
+  const int g_l2 = (int)(l2 / live_bytes);
   int G = env_int("TNB200_CHAIN_G", g_wave > g_l2 ? g_wave : g_l2);
   if (G < 1) G = 1;
   // balanced rounds: ceil(batch / G) of them, sizes differing by at most one sample

@@ -434,6 +434,79 @@ def find_chains(steps, n_inputs, min_len=2):
   return runs
 
 
+def _source(steps, n_inputs, slot):
+  """the slot `slot` is a view of, looking through transposes"""
+  while slot >= n_inputs and steps[slot - n_inputs][0] == "transpose":
+    slot = steps[slot - n_inputs][1]
+  return slot
+
+
+def find_chain_groups(steps, n_inputs, res_slot, shapes):
+  """Candidates for one chained launch each (tnb200_chain_create): lists of step indices in plan order.
+
+  The runs of find_chains go through unchanged.  Among the other contraction steps that are not thin (they contract
+  more than 64 elements), step s continues into step u when u is the only consumer of s's result, that result is not
+  the network's result and no earlier step continues into u.  Runs linked this way (at least two steps long) that do
+  not depend on each other, even transitively, merge into one group: the heads of the four ramps of an MPS
+  contraction interleave in plan order, and one launch runs all four.  A group is launched at its first step, so every
+  operand a member takes from outside the group must be an input (or a view of one) or come from a step before the
+  group's first step; a run that would break this joins no group, and is dropped if it breaks it on its own.
+  `shapes` are the slot shapes of plan_shapes."""
+  runs = find_chains(steps, n_inputs)
+  taken = {i for r in runs for i in r}
+
+  def wide(i):
+    st = steps[i]
+    if i in taken or st[0] not in ("tensordot", "batched"):
+      return False
+    return int(np.prod([shapes[st[1]][a] for a in st[3]] or [1])) > 64
+  ins = [((st[1], st[2]) if st[0] != "transpose" else (st[1],)) for st in steps]
+  users = {}
+  for i, xs in enumerate(ins):
+    for x in xs:
+      users.setdefault(_source(steps, n_inputs, x), set()).add(i)
+  anc = []                                  # steps each step depends on, transitively
+  for i, xs in enumerate(ins):
+    a = set()
+    for x in xs:
+      p = _source(steps, n_inputs, x) - n_inputs
+      if p >= 0:
+        a |= anc[p] | {p}
+    anc.append(a)
+  nxt, has_prev = {}, set()
+  for s in range(len(steps)):
+    u = sorted(users.get(n_inputs + s, ()))
+    if wide(s) and n_inputs + s != res_slot and len(u) == 1 and wide(u[0]) and u[0] not in has_prev:
+      nxt[s] = u[0]
+      has_prev.add(u[0])
+  linked = []
+  for s in sorted(nxt):
+    if s not in has_prev:
+      linked.append([s])
+      while linked[-1][-1] in nxt:
+        linked[-1].append(nxt[linked[-1][-1]])
+
+  def placeable(group):
+    first, members = group[0], set(group)
+    for i in group:
+      for x in ins[i]:
+        p = _source(steps, n_inputs, x) - n_inputs
+        if p >= 0 and p not in members and p >= first:
+          return False
+    return True
+  groups = []
+  for run in linked:
+    for k, g in enumerate(groups):
+      if all(not (anc[i] & set(run)) for i in g) and all(not (anc[i] & set(g)) for i in run) \
+          and placeable(sorted(g + run)):
+        groups[k] = sorted(g + run)
+        break
+    else:
+      if placeable(run):
+        groups.append(run)
+  return sorted(runs + groups)
+
+
 def find_thin_runs(steps, n_inputs, res_slot, shapes, exclude=(), max_len=8):
   """Runs of thin contraction steps linked by dependency (not by index: the ramps of an MPS contraction interleave):
   candidates for one fused launch (tnb200_thin_run_create).  A step is thin when it contracts at most 64 elements;
@@ -593,13 +666,17 @@ class CompiledNetwork:
         users.setdefault(x, []).append(i)
     ring_of = {}
     nring = int(os.environ.get("TNB200_CHAIN_RING", "2"))
+    groups = find_chain_groups(self.steps, n_in, self.res_slot, shp)
     if nring >= 2:
       # Ring slots are shared ONLY between results of identical shape (so sample b occupies the same region in
       # every step that uses the slot) and are handed out round-robin per shape: a slot written by step s is
       # next written by a step s' >= s + 2, which (per sample, through the run's read-after-write counters)
       # cannot start before step s + 1 — the only reader of step s — has finished that sample.  Results of
-      # different per-sample extents never alias (the cfg 2 ramp boundary [256,2,512] -> [512,2,512]).
-      for run in find_chains(self.steps, n_in):
+      # different per-sample extents never alias (the cfg 2 ramp boundary [256,2,512] -> [512,2,512]).  In a
+      # group with branches a member need not wait for the one before it, so nothing there is aliased.
+      for run in groups:
+        if any(n_in + a not in self.steps[b][1:3] for a, b in zip(run, run[1:])):
+          continue
         rings, count = {}, {}
         for k, sid in enumerate(run[:-1]):
           if users.get(n_in + sid, []) == [run[k + 1]] and n_in + sid != self.res_slot:
@@ -622,7 +699,7 @@ class CompiledNetwork:
     self._vals = vals
     chain_of = {}
     self.chains = []
-    pending = find_chains(self.steps, n_in)
+    pending = [list(g) for g in groups]
     if code == L.F32 and be.math_mode in (L.MATH_STRICT, L.MATH_SIMT):
       pending = []            # the chained kernel computes fp32 as TF32: strict fp32 stays on per-step launches
     if be.math_mode == L.MATH_SIMT:
@@ -666,9 +743,11 @@ class CompiledNetwork:
           self.chains.append(ch)
           for sid in run:
             chain_of[sid] = ch
-        elif rc == L.ERR_UNSUPPORTED:
-          k = bad.value if bad.value >= 0 else 0      # split the run around the step the kernel cannot take
+        elif rc == L.ERR_UNSUPPORTED and bad.value >= 0:
+          k = bad.value                               # split the run around the step the kernel cannot take
           pending[:0] = [run[:k], run[k + 1:]]
+        elif rc == L.ERR_UNSUPPORTED:
+          continue                                    # refused as a whole (too few tiles per step): step by step
         else:
           L.check(rc)
     create("chain", pending)
@@ -697,8 +776,7 @@ class CompiledNetwork:
 
   def _producer(self, slot, n_in, pos):
     """position (inside the run `pos`) of the step that produced `slot`, looking through transposes; -1 if outside"""
-    while slot >= n_in and self.steps[slot - n_in][0] == "transpose":
-      slot = self.steps[slot - n_in][1]
+    slot = _source(self.steps, n_in, slot)
     return pos.get(slot - n_in, -1) if slot >= n_in else -1
 
   def _node_io(self, node):
@@ -730,12 +808,13 @@ class CompiledNetwork:
 
   def _run_nodes(self, streams):
     """dependency-aware execution of the node list on `streams` (the structure execute_plan_streams uses); all
-    chained launches share streams[0]: two persistent chain kernels must never wait for each other's SMs."""
+    chained launches share streams[0]: two persistent chain kernels must never wait for each other's SMs.  A node fed
+    only by chained launches takes the next stream in turn: the branches a chain leaves (the ramps after their heads)
+    then go on side by side instead of queueing behind one another on streams[0]."""
     torch = self.backend.torch
     main = torch.cuda.current_stream()
     multi = len(streams) > 1 or streams[0] is not main
-    n_in = len(self.inputs)
-    home, events = {}, {}
+    home, events, from_chain = {}, {}, set()
     if multi:
       for s in streams:
         s.wait_stream(main)
@@ -747,11 +826,13 @@ class CompiledNetwork:
         if src in home:
           home[outs[0]] = home[src]
           events[outs[0]] = events[src]
+          if src in from_chain:
+            from_chain.add(outs[0])
         continue
       produced = [i for i in ins if i in home]
       if node[0] == "chain":
         si = 0
-      elif not produced:
+      elif all(i in from_chain for i in produced):
         si = rr % len(streams)
         rr += 1
       else:
@@ -767,6 +848,8 @@ class CompiledNetwork:
       for o in outs:
         home[o] = si
         events[o] = e
+        if node[0] == "chain":
+          from_chain.add(o)
     if multi:
       for s in streams:
         main.wait_stream(s)

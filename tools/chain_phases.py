@@ -1,18 +1,20 @@
-"""Where the chained zipper kernel spends its time: a per-phase breakdown of the bench's cfg2 chain.
+"""Where the chained GEMM kernel spends its time: a per-phase breakdown of one of the bench's cfg2 chains.
 
 Builds a diagnostic copy of the library with -DTNB200_CHAIN_PHASES into a temporary directory (the default
 library is untouched and carries no timers), builds the cfg2 network (L=64, D=512, bf16, 74 samples, the bench's
-workload), and replays only its chained launch.  Per launch it prints the chain's device time (CUDA events) and,
-averaged over CTAs, the %globaltimer time spent in:
+workload), and replays only one chained launch: `--chain main` (the default) the zipper, `--chain head` the heads of
+the four MPS ramps (plan steps 0-11, four independent branches of three steps).  Per launch it prints the chain's
+device time (CUDA events) and, averaged over CTAs, the %globaltimer time spent in:
   chain_wait   the producer warp spinning on the dependency counters of a tile's operands
   full_wait    the consumers waiting for a ring stage (starved of operands; measured on one consumer thread)
   k_loop       the whole k loop, full_wait included
   epilogue     from the end of the k loop to the point the tile needs nothing more from the consumers
 and, for --G values, the same for other round sizes (TNB200_CHAIN_G).  It also prints the chain's L2 -> SM operand
 feed per launch and its rate over the launch time: the operand bytes the kernel's tiles read, computed from the shapes
-(per pair of M tiles: two 128-row A tiles and one shared B tile of BN rows, each K elements deep), not a counter.
+(per pair of M tiles: its A rows and the B rows of one shared B tile, each K elements deep; rows past the edge of an
+operand are not read), not a counter.
 
-  python tools/chain_phases.py [--G 9 17 19 38] [--reps 20] [--networks 74]
+  python tools/chain_phases.py [--chain main|head] [--G 9 17 19 38] [--reps 20] [--networks 74]
 """
 import argparse
 import ctypes
@@ -31,11 +33,11 @@ BM, BN_16, BN_32 = 128, 256, 128        # the chained kernel's tile (16-bit oper
 
 
 def feed_bytes(m, k, n, esize):
-  """L2 -> SM operand bytes of one sample of one chain step (M x K times K x N, `esize`-byte operands): per N tile and
-  pair of M tiles, the pair's A tiles (one when tiles_m is odd and the pair is the last) and one shared B tile"""
+  """L2 -> SM operand bytes of one sample of one chain step (M x K times K x N, `esize`-byte operands): every N tile
+  reads all M rows of A, every pair of M tiles all N rows of B (each CTA of the pair loads half of a B tile for both)"""
   bn = BN_32 if esize == 4 else BN_16
   tm, tn = -(-m // BM), -(-n // bn)
-  return tn * (tm * BM + -(-tm // 2) * bn) * k * esize
+  return (tn * m + -(-tm // 2) * n) * k * esize
 
 
 def build_phase_lib(out_dir):
@@ -63,6 +65,8 @@ def main():
   ap.add_argument("--G", type=int, nargs="*", default=[], help="round sizes to sweep besides the default")
   ap.add_argument("--reps", type=int, default=20)
   ap.add_argument("--networks", type=int, default=74)
+  ap.add_argument("--chain", choices=["main", "head"], default="main",
+                  help="main: the zipper (the longest chain); head: the ramp heads (the chain that starts the plan)")
   args = ap.parse_args()
   tmp = tempfile.mkdtemp(prefix="tnb200_phases_")
   lib_path = build_phase_lib(tmp)
@@ -104,7 +108,8 @@ def main():
                                   conj_aliases={L + i: i for i in range(L)})
     net.load(kets + list(kets))
     net()
-    ch = max(net.chains, key=lambda c: len(c.steps))
+    chains = [c for c in net.chains if c.api == "chain"]
+    ch = max(chains, key=lambda c: len(c.steps)) if args.chain == "main" else min(chains, key=lambda c: c.steps[0])
     pairwise = [i for i, st in enumerate(net.steps) if st[0] != "transpose"]     # `work` skips transposes
     flops = NB * sum(2.0 * np.prod(work[pairwise.index(s)]) for s in ch.steps)
     feed = NB * sum(feed_bytes(*work[pairwise.index(s)], esize) for s in ch.steps)
@@ -126,7 +131,7 @@ def main():
           "tiles %.1f  (%d CTAs)" % (
               "default" if G is None else G, len(ch.steps), us, flops / us / 1e6, feed / 1e9, feed / us / 1e6,
               "  ".join("%s %.1f" % (n, per[i] / 1e3) for i, n in enumerate(PHASES[:5])), per[5], ctas), flush=True)
-    del net, ch
+    del net, ch, chains
 
 
 if __name__ == "__main__":
