@@ -157,6 +157,16 @@ TNB200_API int32_t tnb200_svd_truncation_count(const tnb200_tensor_t* s, int64_t
                                     int32_t use_error, double max_truncation_error,
                                     int32_t relative, int64_t* keep_dev, void* stream);
 
+/* ---- NumPyBackend.eigh (backends/numpy/numpy_backend.py:165-166, AbstractBackend.eigh
+ *      abstract_backend.py:320-330): np.linalg.eigh of the n x n view `a` (any strides) by parallel two-sided
+ *      block Jacobi.  Only the lower triangle is read (LAPACK's UPLO='L'): the upper triangle is taken as its
+ *      conjugate and the imaginary part of the diagonal is ignored.  w (n, real dtype, ASCENDING) and v (n x n, the
+ *      input dtype, eigenvectors as columns) are preallocated, any strides.  f32 / c64 iterate in double.
+ *      `info` (device int32[4], may be NULL): [0] sweeps used, [1] converged flag.  Synchronises with the host once
+ *      per sweep.  Non-square: TNB200_ERR_INVALID; other dtypes: TNB200_ERR_DTYPE; no convergence: TNB200_ERR_NOCONV. */
+TNB200_API int32_t tnb200_eigh(const tnb200_tensor_t* a, const tnb200_tensor_t* w, const tnb200_tensor_t* v,
+                               int32_t* info_dev, void* stream);
+
 /* ---- a5: decompositions.qr / rq (decompositions.py:77-124).  Reduced QR of the m x n view
  * `a`: q (m x r), r (r x n), r = min(m, n), Householder (LAPACK geqrf sign convention) with the
  * optional non_negative_diagonal phase fix (:91-94).  rq is qr of the conjugate transpose and is

@@ -635,6 +635,24 @@ class CudaB200Backend(_Base):
                                self._stream()))
     return self.reshape(q, list(left) + [r]), self.reshape(rr, [r] + list(right))
 
+  def eigh(self, matrix):
+    """numpy_backend.py:165-166 (np.linalg.eigh) -> (w ascending, v with eigenvectors as columns); reads only the
+    lower triangle, as LAPACK does there."""
+    self._check_type(matrix)
+    self._no_capture("eigh")         # (the sweep loop reads the convergence flag on the host)
+    if matrix.ndim != 2:
+      raise NotImplementedError("eigh expects a 2-D tensor (stacks of matrices are not implemented), got shape {}"
+                                .format(tuple(matrix.shape)))
+    if matrix.code in (L.I32, L.I64, L.F16, L.BF16):
+      raise TypeError("eigh needs a float32/float64/complex tensor")
+    n, m = matrix.shape
+    if n != m:
+      raise ValueError("eigh needs a square matrix, got shape {}".format((n, m)))
+    w = self._new((n,), T.real_code(matrix.code))
+    v = self._new((n, n), matrix.code)
+    L.check(self.lib.tnb200_eigh(matrix.ref(), w.ref(), v.ref(), None, self._stream()))
+    return w, v
+
   def rq(self, tensor, pivot_axis=-1, non_negative_diagonal=False):
     """decompositions.py:101-124: QR of the conjugate transpose, then conjugate back."""
     self._check_type(tensor)
