@@ -167,6 +167,18 @@ TNB200_API int32_t tnb200_svd_truncation_count(const tnb200_tensor_t* s, int64_t
 TNB200_API int32_t tnb200_eigh(const tnb200_tensor_t* a, const tnb200_tensor_t* w, const tnb200_tensor_t* v,
                                int32_t* info_dev, void* stream);
 
+/* ---- NumPyBackend.eigs (backends/numpy/numpy_backend.py:216-298, which hands off to scipy's ARPACK): one Arnoldi
+ *      step's orthogonalisation, two passes of classical Gram-Schmidt (CGS2) of w against rows 0..j of the Krylov
+ *      basis v, a row-major matrix view (rows >= j + 2, contiguous rows, any row stride; row i = Krylov vector i).
+ *      Writes the normalised result into row j+1 of v, h_dev[0..j] = V[0..j]^H w (the sum of both passes) and
+ *      h_dev[j+1] = beta, the norm before normalising.  h_dev holds j + 2 values of the double-precision form of the
+ *      basis dtype (f64 for f64 / f32, c128 for c128 / c64).  w (contiguous, n elements, the basis dtype) is only
+ *      read.  If beta <= 16 sqrt(j + 2) eps(dtype) ||w||, w lies in span(V) to rounding: row j+1 is written as zeros
+ *      and beta as 0.  f64 / c128 / f32 / c64, accumulation in double, j + 1 <= 1024 (TNB200_ERR_UNSUPPORTED above).
+ *      Four launches per call for any j and n, three reads of rows 0..j; no host synchronisation. */
+TNB200_API int32_t tnb200_arnoldi_orth(const tnb200_tensor_t* v, int32_t j, const tnb200_tensor_t* w, void* h_dev,
+                                       void* stream);
+
 /* ---- a5: decompositions.qr / rq (decompositions.py:77-124).  Reduced QR of the m x n view
  * `a`: q (m x r), r (r x n), r = min(m, n), Householder (LAPACK geqrf sign convention) with the
  * optional non_negative_diagonal phase fix (:91-94).  rq is qr of the conjugate transpose and is

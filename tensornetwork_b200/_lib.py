@@ -66,6 +66,7 @@ SIGNATURES = {
     "tnb200_svd": (_i32, [_P, _P, _P, _P, _vp, _vp]),
     "tnb200_svd_truncation_count": (_i32, [_P, _i64, _i32, _dbl, _i32, _vp, _vp]),
     "tnb200_eigh": (_i32, [_P, _P, _P, _vp, _vp]),
+    "tnb200_arnoldi_orth": (_i32, [_P, _i32, _P, _vp, _vp]),
     "tnb200_qr": (_i32, [_P, _P, _P, _i32, _vp]),
     "tnb200_blocksparse_maps": (_i32, [_i32, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _i64, _i32, _vp, _i64, _vp, _vp]),
     "tnb200_svd_batched": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),

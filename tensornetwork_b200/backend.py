@@ -672,6 +672,18 @@ class CudaB200Backend(_Base):
     return lanczos.eigsh_lanczos(self, A, args, initial_state, shape, dtype, num_krylov_vecs,
                                  numeig, tol, delta, ndiag, reorthogonalize)
 
+  # ------------------------------------------------------------------ Arnoldi
+  def eigs(self, A, args=None, initial_state=None, shape=None, dtype=None, num_krylov_vecs=50, numeig=6, tol=1e-8,
+           which='LR', maxiter=None):
+    """numpy_backend.py:216-298 (scipy's ARPACK there): implicitly restarted Arnoldi with exact shifts.  Returns
+    (eta, eigvecs): eta a 1-D device tensor of `numeig` complex eigenvalues (c128 for f64 / c128 input, c64 for f32 /
+    c64), best first under `which` ('LM', 'SM', 'LR', 'SR'), Im > 0 first within a conjugate pair; eigvecs a list of
+    `numeig` complex device tensors of initial_state's shape with unit 2-norm.  For a real operator the basis stays
+    real, and a real eigenvalue and its vector have imaginary parts exactly 0."""
+    self._no_capture("eigs")         # (beta is read on the host at every step)
+    from . import arnoldi  # pylint: disable=import-outside-toplevel
+    return arnoldi.eigs(self, A, args, initial_state, shape, dtype, num_krylov_vecs, numeig, tol, which, maxiter)
+
 
 def register():
   """Insert the backend into the reference's registry (backend_factory.py:22-28)."""
