@@ -47,7 +47,9 @@ typedef enum {
   TNB200_C64 = 4,   /* interleaved (re, im) float  */
   TNB200_C128 = 5,  /* interleaved (re, im) double */
   TNB200_I32 = 6,
-  TNB200_I64 = 7
+  TNB200_I64 = 7,
+  TNB200_BOOL = 8   /* one byte, 0 or 1: a mask.  Only tnb200_compare (output) and tnb200_index_update (mask)
+                       accept it; every other entry point refuses a bool descriptor. */
 } tnb200_dtype_t;
 
 /* A strided view of device memory.  Strides are in ELEMENTS (like torch), may be 0
@@ -119,6 +121,23 @@ TNB200_API int32_t tnb200_scale_by_device_scalar(const tnb200_tensor_t* x, const
 TNB200_API int32_t tnb200_axpy(const tnb200_tensor_t* x, const tnb200_tensor_t* y, double alpha_re,
                     double alpha_im, const void* alpha_dev, double sign, void* stream);
 TNB200_API int32_t tnb200_fill(const tnb200_tensor_t* c, double re, double im, void* stream);
+/* ---- elementwise comparison masks (numpy's `a <= b` etc., used by InfiniteMPS.canonicalize,
+ *      matrixproductstates/infinite_mps.py:237,263).  c (TNB200_BOOL) = a (op) b with the operand conventions of
+ *      tnb200_binary: same ndim and shape, broadcasting by 0-strides, a and b of one dtype.  IEEE semantics: any
+ *      comparison with NaN is false.  f64 / f32 / f16 / bf16 / i32 / i64; complex: TNB200_ERR_DTYPE. */
+typedef enum { TNB200_LT = 0, TNB200_LE = 1, TNB200_GT = 2, TNB200_GE = 3 } tnb200_cmpop_t;
+TNB200_API int32_t tnb200_compare(int32_t op, const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200_tensor_t* c,
+                                  void* stream);
+/* ---- NumPyBackend.index_update (numpy_backend.py:548-552: t = copy(a); t[mask] = value):
+ *      out = where(mask, value, a) in one strided launch.  mask (TNB200_BOOL) has a's shape (0-strides broadcast it) or
+ *      is NULL, which selects every element.  The value is (re, im) from the host, or, when value_dev is not NULL, the
+ *      scalar of dtype value_dtype read on the device (no host sync; an i64 scalar stored into an i64 tensor is copied
+ *      exactly, so integers beyond 2^53, which a double rounds, go that way).  It is cast to a's dtype as numpy casts: a float
+ *      stored into an integer tensor is truncated toward zero; a complex value into a real tensor is TNB200_ERR_DTYPE
+ *      (host values: im != 0).  out has a's shape and dtype, any strides. */
+TNB200_API int32_t tnb200_index_update(const tnb200_tensor_t* a, const tnb200_tensor_t* mask, double re, double im,
+                                       const void* value_dev, int32_t value_dtype, const tnb200_tensor_t* out,
+                                       void* stream);
 /* c[i, j] = (j - i == k) — NumPyBackend.eye :110-116 */
 TNB200_API int32_t tnb200_eye(const tnb200_tensor_t* c, int64_t k, void* stream);
 /* standard normal fill (Philox4x32-10 + Box-Muller), NumPyBackend.randn :132-144; complex
@@ -185,6 +204,36 @@ TNB200_API int32_t tnb200_arnoldi_orth(const tnb200_tensor_t* v, int32_t j, cons
  * composed by the adapter. */
 TNB200_API int32_t tnb200_qr(const tnb200_tensor_t* a, const tnb200_tensor_t* q, const tnb200_tensor_t* r,
                   int32_t non_negative_diagonal, void* stream);
+
+/* ---- LU with partial pivoting: LAPACK getrf, as scipy.linalg.lu_factor computes it; the factorisation behind
+ *      NumPyBackend.inv (numpy_backend.py:554-558).  lu_factor factors the n x n view `a` (any strides) and writes the
+ *      packed factors into `lu` (n x n, any strides): unit L strictly below the diagonal, U on and above it.
+ *      piv_dev[n] (device int32) receives the 0-based row interchanges in LAPACK's order (row i was swapped with row
+ *      piv[i], i <= piv[i] < n); the pivot of column j is the FIRST row of largest |x| (real) or |re| + |im| (complex),
+ *      with NaN treated as reference BLAS idamax / izamax treat it: a NaN on the diagonal stays the pivot, a NaN below
+ *      it is never chosen, and the NaNs propagate through the factors.  Complex pivots are divided by without forming
+ *      |x|^2 (Smith's algorithm), so the whole double range is safe.
+ *      info_dev[0] (device int32) is set to 0, or to 1 + the index of the first pivot that is exactly zero (LAPACK's
+ *      info); the factorisation still completes, as in LAPACK.
+ *      Right-looking and blocked, panels of 32 columns, four launches per panel and none per column:
+ *        - the panel: ONE cluster of 8 CTAs; its rows are dealt to the CTAs and held in shared memory while they fit
+ *          (n - j0 <= ~6900 rows for f64, ~3400 for c128; above that the same kernel works on the panel in global
+ *          memory, where it stays L2-resident).  Per column one cluster-wide exchange through distributed shared
+ *          memory carries each CTA's pivot candidate (|x|, index, row) and the diagonal row; the swap, the scale and
+ *          the rank-1 update of the panel are then local;
+ *        - the row interchanges left and right of the panel (laswp), the U12 triangular solve, and the trailing update
+ *          A22 -= L21 U12.
+ *      f64 runs the trailing update on the FP64 tensor pipe (DMMA m8n8k4); c128 runs it with CUDA-core FMA.
+ *      f32 / c64 are widened to f64 / c128, factored, and rounded back.  Other dtypes: TNB200_ERR_DTYPE; not square:
+ *      TNB200_ERR_INVALID; n = 0: no-op.  Does not synchronise with the host. */
+TNB200_API int32_t tnb200_lu_factor(const tnb200_tensor_t* a, const tnb200_tensor_t* lu, int32_t* piv_dev,
+                                    int32_t* info_dev, void* stream);
+/* ---- NumPyBackend.inv (numpy_backend.py:554-558, np.linalg.inv): x = a^-1, x preallocated (n x n, any strides).
+ *      The factorisation above, then a blocked solve against the permuted identity (forward with unit L, backward with
+ *      U, 32 rows per step: a triangular solve and one update launch each, the update on DMMA for f64).  Launches:
+ *      at most 8 ceil(n / 32) + 8.  info_dev[0] as for tnb200_lu_factor: nonzero means the matrix is singular and x
+ *      holds no inverse.  Same dtypes and errors as tnb200_lu_factor.  Does not synchronise with the host. */
+TNB200_API int32_t tnb200_inv(const tnb200_tensor_t* a, const tnb200_tensor_t* x, int32_t* info_dev, void* stream);
 
 /* ---- a11: block_sparse.tensordot per-sector loop (block_sparse/blocksparsetensor.py:1094-1101).
  * For each sector q: C.data[c_map[q]] = A.data[a_map[q]].reshape(m_q,k_q) @ B.data[b_map[q]]

@@ -346,7 +346,8 @@ class CudaB200Backend(_Base):
   def imag(self, tensor):
     return self._unary(L.IMAG, tensor, T.real_code(tensor.code))
 
-  def _binary(self, op, x, y):
+  def _operands(self, x, y, int_to_float=False):
+    """The two operands of an elementwise op as tensors of one promoted dtype, expanded to the broadcast shape."""
     if isinstance(x, B200Tensor):
       y = self._as_tensor(y, x.code)
     elif isinstance(y, B200Tensor):
@@ -355,7 +356,7 @@ class CudaB200Backend(_Base):
       x = self._as_tensor(x)
       y = self._as_tensor(y, x.code)
     code = self._promote(x.code, y.code)
-    if op == L.DIV and code in (L.I32, L.I64):
+    if int_to_float and code in (L.I32, L.I64):
       code = L.F64
     x, y = self.astype(x, code), self.astype(y, code)
     try:
@@ -365,8 +366,84 @@ class CudaB200Backend(_Base):
           x.shape, y.shape)) from e
     xe = x if x.shape == shape else B200Tensor(x.t.expand(shape), code)
     ye = y if y.shape == shape else B200Tensor(y.t.expand(shape), code)
+    return xe, ye, shape, code
+
+  def _binary(self, op, x, y):
+    xe, ye, shape, code = self._operands(x, y, int_to_float=op == L.DIV)
     out = self._new(shape, code)
     L.check(self.lib.tnb200_binary(op, xe.ref(), ye.ref(), out.ref(), self._stream()))
+    return out
+
+  def compare(self, op, x, y):
+    """x (op) y elementwise (op: _lib.LT / LE / GT / GE) -> a bool mask of the broadcast shape, computed on the device
+    with no host sync; operands are promoted as for arithmetic.  Complex operands raise TypeError (no ordering)."""
+    xe, ye, shape, _ = self._operands(x, y)
+    out = self._new(shape, L.BOOL)
+    L.check(self.lib.tnb200_compare(op, xe.ref(), ye.ref(), out.ref(), self._stream()))
+    return out
+
+  def index_update(self, tensor, mask, assignee):
+    """numpy_backend.py:548-552 (`t = np.copy(tensor); t[mask] = assignee`) -> a new tensor; the input is untouched.
+    mask: a bool device mask, a host numpy bool array, or a Python / numpy bool (True sets everything, False nothing),
+    of tensor's shape or a leading prefix of it (which selects whole sub-blocks).  assignee: a Python / numpy scalar, or
+    a one-element device tensor read on the device (no host sync), cast as numpy casts."""
+    self._check_type(tensor)
+    if isinstance(mask, (bool, np.bool_)) or (isinstance(mask, np.ndarray) and mask.ndim == 0 and mask.dtype == bool):
+      if not bool(mask):
+        return self.copy(tensor)
+      mask = None
+    elif isinstance(mask, np.ndarray):
+      if mask.dtype != bool:
+        raise IndexError("index_update needs a boolean mask, got an array of dtype {}".format(mask.dtype))
+      mask = self.convert_to_tensor(mask)
+    elif not isinstance(mask, B200Tensor) or mask.code != L.BOOL:
+      raise IndexError("index_update needs a boolean mask (a bool tensor, a numpy bool array or a bool), got {!r}"
+                       .format(mask))
+    if mask is not None:
+      nd = mask.ndim
+      if nd > tensor.ndim or tuple(mask.shape) != tuple(tensor.shape[:nd]):
+        raise IndexError("boolean index of shape {} does not match the indexed array of shape {}"
+                         .format(tuple(mask.shape), tuple(tensor.shape)))
+      if nd < tensor.ndim:
+        mask = B200Tensor(mask.t.reshape(tuple(mask.shape) + (1,) * (tensor.ndim - nd)).expand(tensor.shape), L.BOOL)
+    real_target = not T.is_complex_code(tensor.code)
+    re = im = 0.0
+    vdev, vcode = None, 0
+    if isinstance(assignee, B200Tensor):
+      if assignee.size != 1:
+        raise NotImplementedError("index_update assigns one value: a scalar or a one-element tensor (got shape {}); "
+                                  "one value per selected element is not supported".format(assignee.shape))
+      if real_target and T.is_complex_code(assignee.code):
+        raise TypeError("cannot assign a complex value to a {} tensor".format(tensor.dtype))
+      if not assignee.t.is_contiguous():
+        assignee = self.copy(assignee)
+      vdev, vcode = assignee.t.data_ptr(), assignee.code
+    elif np.ndim(assignee) == 0 and not isinstance(assignee, (str, bytes)):
+      v = np.asarray(assignee).item()
+      if isinstance(v, complex):
+        if real_target:
+          raise TypeError("cannot assign a complex value to a {} tensor".format(tensor.dtype))
+        re, im = v.real, v.imag
+      elif tensor.code in (L.I32, L.I64):
+        iv = int(v)                         # numpy truncates a float toward zero
+        bits = 32 if tensor.code == L.I32 else 64
+        if not -(1 << (bits - 1)) <= iv < (1 << (bits - 1)):
+          if isinstance(assignee, int):     # numpy refuses an out-of-range Python int, and wraps a numpy integer
+            raise OverflowError("Python integer {} out of bounds for {}".format(iv, tensor.dtype))
+          iv = (iv + (1 << (bits - 1))) % (1 << bits) - (1 << (bits - 1))
+        if abs(iv) <= 1 << 53:
+          re = float(iv)                    # exact as a double
+        else:                               # beyond 2^53 a double rounds: hand the kernel an exact int64 scalar
+          staged = self.convert_to_tensor(np.array(iv, dtype=np.int64))
+          vdev, vcode = staged.t.data_ptr(), L.I64
+      else:
+        re = float(v)
+    else:
+      raise NotImplementedError("index_update assigns one value: a Python / numpy scalar or a one-element tensor; an "
+                                "array of values (one per selected element) is not supported")
+    out = self._new(tensor.shape, tensor.code)
+    L.check(self.lib.tnb200_index_update(tensor.ref(), None if mask is None else mask.ref(), re, im, vdev, vcode,
+                                         out.ref(), self._stream()))
     return out
 
   def addition(self, tensor1, tensor2):
@@ -652,6 +729,31 @@ class CudaB200Backend(_Base):
     v = self._new((n, n), matrix.code)
     L.check(self.lib.tnb200_eigh(matrix.ref(), w.ref(), v.ref(), None, self._stream()))
     return w, v
+
+  def inv(self, matrix):
+    """numpy_backend.py:554-558 (np.linalg.inv): LU with partial pivoting (tnb200_inv).  Integer input is inverted in
+    float64, as numpy does.  Reads LAPACK's info once after the launch: a zero pivot raises LinAlgError."""
+    self._check_type(matrix)
+    if matrix.ndim > 2:
+      raise ValueError("input to numpy backend method `inv` has shape {}. Only matrices are supported."
+                       .format(matrix.shape))
+    if matrix.ndim < 2:
+      raise np.linalg.LinAlgError("{}-dimensional array given. Array must be at least two-dimensional"
+                                  .format(matrix.ndim))
+    n, m = matrix.shape
+    if n != m:
+      raise np.linalg.LinAlgError("Last 2 dimensions of the array must be square")
+    if matrix.code in (L.F16, L.BF16):
+      raise TypeError("array type {} is unsupported in linalg".format(matrix.dtype))
+    self._no_capture("inv")          # (info is read on the host)
+    if matrix.code in (L.I32, L.I64):
+      matrix = self.astype(matrix, L.F64)
+    x = self._new((n, n), matrix.code)
+    info = self.torch.zeros(1, dtype=self.torch.int32, device=self.device)
+    L.check(self.lib.tnb200_inv(matrix.ref(), x.ref(), info.data_ptr(), self._stream()))
+    if int(info.item()) != 0:
+      raise np.linalg.LinAlgError("Singular matrix")
+    return x
 
   def rq(self, tensor, pivot_axis=-1, non_negative_diagonal=False):
     """decompositions.py:101-124: QR of the conjugate transpose, then conjugate back."""

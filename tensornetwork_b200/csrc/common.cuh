@@ -63,8 +63,8 @@ inline int dtype_size(int dt) {
 }
 inline bool dtype_is_complex(int dt) { return dt == TNB200_C64 || dt == TNB200_C128; }
 inline const char* dtype_name(int dt) {
-  static const char* n[] = {"f64", "f32", "f16", "bf16", "c64", "c128", "i32", "i64"};
-  return (dt >= 0 && dt < 8) ? n[dt] : "?";
+  static const char* n[] = {"f64", "f32", "f16", "bf16", "c64", "c128", "i32", "i64", "bool"};
+  return (dt >= 0 && dt < 9) ? n[dt] : "?";
 }
 
 inline int num_sms() {

@@ -627,6 +627,106 @@ static int gather_t(const void* src, const int64_t* idx, void* dst, int64_t n, i
   return 0;
 }
 
+// ------------------------------------------------------------------ comparison masks / index_update
+// values compared in their own type (int64 stays exact, NaN compares false), 16-bit floats through float
+__device__ inline double cmp_val(double x) { return x; }
+__device__ inline float cmp_val(float x) { return x; }
+__device__ inline float cmp_val(__half x) { return __half2float(x); }
+__device__ inline float cmp_val(__nv_bfloat16 x) { return __bfloat162float(x); }
+__device__ inline int32_t cmp_val(int32_t x) { return x; }
+__device__ inline long long cmp_val(long long x) { return x; }
+
+template <typename T>
+__global__ void compare_kernel(int op, const T* __restrict__ a, const T* __restrict__ b, uint8_t* __restrict__ c, DevModes m,
+                               int64_t total) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t o0, o1, o2;
+    mode_offsets3(m, i, o0, o1, o2);
+    const auto x = cmp_val(a[o0]), y = cmp_val(b[o1]);
+    bool r;
+    switch (op) {
+      case TNB200_LT: r = x < y; break;
+      case TNB200_LE: r = x <= y; break;
+      case TNB200_GT: r = x > y; break;
+      default: r = x >= y; break;
+    }
+    c[o2] = r ? 1 : 0;
+  }
+}
+template <typename T>
+static int compare_t(int op, const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200_tensor_t* c, cudaStream_t st) {
+  DevModes dm; int64_t total;
+  int rc = build_modes(a, b, c, dm, total);
+  if (rc) return rc;
+  if (total == 0) return 0;
+  compare_kernel<T><<<grid_for(total), 256, 0, st>>>(op, (const T*)a->data, (const T*)b->data, (uint8_t*)c->data, dm, total);
+  TNB_LAUNCH_CHECK();
+  count_launch();
+  return 0;
+}
+
+// numpy's casting of an assigned value: floats stored into an integer tensor truncate toward zero
+template <typename T> __device__ inline void st_assign(T* p, ZV v) { stv<T>(p, v); }
+template <> __device__ inline void st_assign<int32_t>(int32_t* p, ZV v) { *p = (int32_t)(long long)v.re; }
+template <> __device__ inline void st_assign<long long>(long long* p, ZV v) { *p = (long long)v.re; }
+
+__device__ inline ZV ld_dtype(const void* p, int dt) {
+  switch (dt) {
+    case TNB200_F64: return ld<double>((const double*)p);
+    case TNB200_F32: return ld<float>((const float*)p);
+    case TNB200_F16: return ld<__half>((const __half*)p);
+    case TNB200_BF16: return ld<__nv_bfloat16>((const __nv_bfloat16*)p);
+    case TNB200_C64: return ld<cuFloatComplex>((const cuFloatComplex*)p);
+    case TNB200_C128: return ld<cuDoubleComplex>((const cuDoubleComplex*)p);
+    case TNB200_I32: return ld<int32_t>((const int32_t*)p);
+    case TNB200_I64: return ld<long long>((const long long*)p);
+    default: return ZV{(double)*(const uint8_t*)p, 0.0};
+  }
+}
+
+// a value read on the device, cast to T; an integer source into an int64 tensor is copied exactly
+template <typename T> __device__ inline T assign_from_dev(const void* p, int dt) { T v; st_assign<T>(&v, ld_dtype(p, dt)); return v; }
+template <> __device__ inline long long assign_from_dev<long long>(const void* p, int dt) {
+  if (dt == TNB200_I64) return *(const long long*)p;
+  if (dt == TNB200_I32) return *(const int32_t*)p;
+  return (long long)ld_dtype(p, dt).re;
+}
+
+// out = where(mask, value, a); mask == NULL selects everything
+template <typename T>
+__global__ void index_update_kernel(const T* __restrict__ a, const uint8_t* __restrict__ mask, T* __restrict__ out, DevModes m,
+                                    int64_t total, ZV value, const void* value_dev, int value_dt) {
+  T vt;
+  if (value_dev) vt = assign_from_dev<T>(value_dev, value_dt);
+  else st_assign<T>(&vt, value);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t o0, o1, o2;
+    mode_offsets3(m, i, o0, o1, o2);
+    out[o2] = (mask == nullptr || mask[o1]) ? vt : a[o0];
+  }
+}
+template <typename T>
+static int index_update_t(const tnb200_tensor_t* a, const tnb200_tensor_t* mask, ZV value, const void* value_dev, int value_dt,
+                          const tnb200_tensor_t* out, cudaStream_t st) {
+  DevModes dm; int64_t total;
+  int rc = mask ? build_modes(a, mask, out, dm, total) : build_modes(a, out, nullptr, dm, total);
+  if (rc) return rc;
+  if (!mask) for (int i = 0; i < kDevModes; ++i) { dm.s2[i] = dm.s1[i]; dm.s1[i] = 0; }
+  if (total == 0) return 0;
+  index_update_kernel<T><<<grid_for(total), 256, 0, st>>>((const T*)a->data, mask ? (const uint8_t*)mask->data : nullptr,
+                                                          (T*)out->data, dm, total, value, value_dev, value_dt);
+  TNB_LAUNCH_CHECK();
+  count_launch();
+  return 0;
+}
+
+// a descriptor of the mask dtype: valid_tensor() refuses TNB200_BOOL on purpose, so only these entry points take it
+static bool valid_mask(const tnb200_tensor_t* t) {
+  if (!t || t->ndim < 0 || t->ndim > TNB200_MAX_NDIM || t->dtype != TNB200_BOOL) return false;
+  for (int i = 0; i < t->ndim; ++i) if (t->shape[i] < 0) return false;
+  return true;
+}
+
 static int real_dtype(int dt) {
   if (dt == TNB200_C128) return TNB200_F64;
   if (dt == TNB200_C64) return TNB200_F32;
@@ -695,6 +795,38 @@ int32_t tnb200_axpy(const tnb200_tensor_t* x, const tnb200_tensor_t* y, double a
 int32_t tnb200_fill(const tnb200_tensor_t* c, double re, double im, void* stream) {
   TNB_REQUIRE(valid_tensor(c), TNB200_ERR_INVALID, "fill: invalid tensor descriptor");
   TNB_DISPATCH_DTYPE(c->dtype, fill_t, c, ZV{re, im}, (cudaStream_t)stream);
+}
+
+int32_t tnb200_compare(int32_t op, const tnb200_tensor_t* a, const tnb200_tensor_t* b, const tnb200_tensor_t* c, void* stream) {
+  TNB_REQUIRE(valid_tensor(a) && valid_tensor(b) && valid_mask(c), TNB200_ERR_INVALID,
+              "compare: invalid tensor descriptor (the output must be a bool mask)");
+  TNB_REQUIRE(a->ndim == b->ndim && a->ndim == c->ndim, TNB200_ERR_INVALID, "compare: rank mismatch");
+  TNB_REQUIRE(a->dtype == b->dtype, TNB200_ERR_DTYPE, "compare: dtype mismatch");
+  TNB_REQUIRE(op >= TNB200_LT && op <= TNB200_GE, TNB200_ERR_INVALID, "compare: bad op %d", op);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (a->dtype) {
+    case TNB200_F64: return compare_t<double>(op, a, b, c, st);
+    case TNB200_F32: return compare_t<float>(op, a, b, c, st);
+    case TNB200_F16: return compare_t<__half>(op, a, b, c, st);
+    case TNB200_BF16: return compare_t<__nv_bfloat16>(op, a, b, c, st);
+    case TNB200_I32: return compare_t<int32_t>(op, a, b, c, st);
+    case TNB200_I64: return compare_t<long long>(op, a, b, c, st);
+    default: set_error("compare: complex values are not ordered (%s)", dtype_name(a->dtype)); return TNB200_ERR_DTYPE;
+  }
+}
+
+int32_t tnb200_index_update(const tnb200_tensor_t* a, const tnb200_tensor_t* mask, double re, double im, const void* value_dev,
+                            int32_t value_dtype, const tnb200_tensor_t* out, void* stream) {
+  TNB_REQUIRE(valid_tensor(a) && valid_tensor(out) && (mask == nullptr || valid_mask(mask)), TNB200_ERR_INVALID,
+              "index_update: invalid tensor descriptor (the mask must be bool)");
+  TNB_REQUIRE(a->ndim == out->ndim && (mask == nullptr || mask->ndim == a->ndim), TNB200_ERR_INVALID, "index_update: rank mismatch");
+  TNB_REQUIRE(a->dtype == out->dtype, TNB200_ERR_DTYPE, "index_update: dtype mismatch");
+  const bool cplx_value = value_dev ? dtype_is_complex(value_dtype) : im != 0.0;
+  TNB_REQUIRE(!value_dev || (value_dtype >= TNB200_F64 && value_dtype <= TNB200_BOOL), TNB200_ERR_DTYPE,
+              "index_update: bad value dtype %d", value_dtype);
+  TNB_REQUIRE(dtype_is_complex(a->dtype) || !cplx_value, TNB200_ERR_DTYPE,
+              "index_update: cannot assign a complex value to a %s tensor", dtype_name(a->dtype));
+  TNB_DISPATCH_DTYPE(a->dtype, index_update_t, a, mask, ZV{re, im}, value_dev, value_dtype, out, (cudaStream_t)stream);
 }
 
 int32_t tnb200_eye(const tnb200_tensor_t* c, int64_t k, void* stream) {

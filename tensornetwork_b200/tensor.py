@@ -33,7 +33,7 @@ bfloat16 = BFloat16()
 
 _NP2CODE = {np.dtype(np.float64): L.F64, np.dtype(np.float32): L.F32, np.dtype(np.float16): L.F16,
             np.dtype(np.complex64): L.C64, np.dtype(np.complex128): L.C128,
-            np.dtype(np.int32): L.I32, np.dtype(np.int64): L.I64}
+            np.dtype(np.int32): L.I32, np.dtype(np.int64): L.I64, np.dtype(bool): L.BOOL}
 _CODE2NP = {v: k for k, v in _NP2CODE.items()}
 _CODE2NP[L.BF16] = bfloat16
 _REAL_OF = {L.C64: L.F32, L.C128: L.F64}
@@ -49,7 +49,7 @@ def _init_torch():
     _torch = torch
     _CODE2TORCH = {L.F64: torch.float64, L.F32: torch.float32, L.F16: torch.float16,
                    L.BF16: torch.bfloat16, L.C64: torch.complex64, L.C128: torch.complex128,
-                   L.I32: torch.int32, L.I64: torch.int64}
+                   L.I32: torch.int32, L.I64: torch.int64, L.BOOL: torch.bool}
     _TORCH2CODE = {v: k for k, v in _CODE2TORCH.items()}
   return _torch
 
@@ -184,18 +184,26 @@ class B200Tensor:
   def __repr__(self):
     return "B200Tensor(shape={}, dtype={}, device={})".format(self.shape, self.dtype, self.t.device)
 
-  # comparisons of 0-d results against python numbers (Lanczos `abs(norm) < delta`)
+  # A one-element tensor against a host scalar or another one-element tensor compares on the host and returns a Python
+  # bool (Lanczos `abs(norm) < delta`).  Anything else compares on the device and returns a bool mask of the broadcast
+  # shape, without a host sync (infinite_mps.py:237 `mask = eigvals <= cutoff`).  There is deliberately no __eq__:
+  # defining it would make the handle unhashable.
+  def _compare(self, o, op, host):
+    if self.t.numel() == 1 and (o.size == 1 if isinstance(o, B200Tensor) else np.ndim(o) == 0):
+      return host(self.item(), _scalar(o))
+    return _be().compare(op, self, o)
+
   def __lt__(self, o):
-    return self.item() < _scalar(o)
+    return self._compare(o, L.LT, lambda x, y: x < y)
 
   def __le__(self, o):
-    return self.item() <= _scalar(o)
+    return self._compare(o, L.LE, lambda x, y: x <= y)
 
   def __gt__(self, o):
-    return self.item() > _scalar(o)
+    return self._compare(o, L.GT, lambda x, y: x > y)
 
   def __ge__(self, o):
-    return self.item() >= _scalar(o)
+    return self._compare(o, L.GE, lambda x, y: x >= y)
 
   def __abs__(self):
     return _be().abs(self)
