@@ -27,16 +27,31 @@ def _order(theta, which):
   return np.lexsort((-theta.imag, key))
 
 
-class _Krylov:
-  """The (m + 1) x n basis in two device buffers (rows padded to 16 bytes) and the device Hessenberg columns."""
+def _matvec_result(be, w, shape, n, code, who):
+  """A matvec's result w as a contiguous length-n vector in the basis dtype.  w must be a `B200Tensor` of the
+  operand's shape; a real problem's matvec must not return a complex tensor (other dtypes are converted)."""
+  if not isinstance(w, B200Tensor):
+    raise TypeError("{}: the matvec returned {}, expected a `B200Tensor`".format(who, type(w)))
+  if tuple(w.shape) != shape:
+    raise ValueError("{}: the matvec returned shape {}, expected {}".format(who, tuple(w.shape), shape))
+  if w.code != code:
+    if not T.is_complex_code(code) and T.is_complex_code(w.code):
+      raise TypeError("{}: the matvec of a real problem returned a complex tensor".format(who))
+    w = be.astype(w, code)
+  return be.reshape(be.contiguous(w), (n,))
 
-  def __init__(self, be, m, n, code):
+
+class _Krylov:
+  """The (m + 1) x n basis in `nbufs` device buffers (rows padded to 16 bytes) and the device Hessenberg columns.
+  eigs keeps two buffers, so that a restart can compress one basis into the other; gmres needs one."""
+
+  def __init__(self, be, m, n, code, nbufs):
     self.be, self.m, self.n, self.code = be, m, n, code
     torch = be.torch
     tdt = T.code_to_torch(code)
     pad = 16 // np.dtype(T.code_to_np(code)).itemsize
     ldv = -(-n // pad) * pad
-    self.bufs = [torch.empty((m + 1, ldv), dtype=tdt, device=be.device) for _ in range(2)]
+    self.bufs = [torch.empty((m + 1, ldv), dtype=tdt, device=be.device) for _ in range(nbufs)]
     self.V = [B200Tensor(b[:, :n], code) for b in self.bufs]
     self.cur = 0
     self.acc_torch = torch.complex128 if T.is_complex_code(code) else torch.float64
@@ -113,7 +128,7 @@ def eigs(be, A, args=None, initial_state=None, shape=None, dtype=None, num_krylo
   eps23 = eps ** (2.0 / 3.0)
   acc_np = np.float64 if real else np.complex128
 
-  K = _Krylov(be, m, n, code)
+  K = _Krylov(be, m, n, code, 2)
   row0 = K.row(0)
   L.check(be.lib.tnb200_copy(be.reshape(initial_state, (n,)).ref(), row0.ref(), 0, be._stream()))
   nrm = float(be.norm(row0).item())
@@ -125,15 +140,7 @@ def eigs(be, A, args=None, initial_state=None, shape=None, dtype=None, num_krylo
   def matvec(j):
     w = A(be.reshape(K.row(j), shape), *args)
     K.matvecs += 1
-    if not isinstance(w, B200Tensor):
-      raise TypeError("eigs: the matvec returned {}, expected a `B200Tensor`".format(type(w)))
-    if tuple(w.shape) != shape:
-      raise ValueError("eigs: the matvec returned shape {}, expected {}".format(tuple(w.shape), shape))
-    if w.code != code:
-      if real and T.is_complex_code(w.code):
-        raise TypeError("eigs: the matvec of a real problem returned a complex tensor")
-      w = be.astype(w, code)
-    return be.reshape(be.contiguous(w), (n,))
+    return _matvec_result(be, w, shape, n, code, "eigs")
 
   H = np.zeros((m + 1, m), dtype=acc_np)
   p = 0

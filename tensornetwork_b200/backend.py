@@ -786,6 +786,30 @@ class CudaB200Backend(_Base):
     from . import arnoldi  # pylint: disable=import-outside-toplevel
     return arnoldi.eigs(self, A, args, initial_state, shape, dtype, num_krylov_vecs, numeig, tol, which, maxiter)
 
+  def gmres(self, A_mv, b, A_args=None, A_kwargs=None, x0=None, tol=1e-5, atol=None, num_krylov_vectors=20,
+            maxiter=1, M=None):
+    """abstract_backend.py:478-615: restarted GMRES for A x = b, A given by `A_mv(x, *A_args, **A_kwargs)` on tensors
+    of b's shape.  Returns (x, info): x a device tensor of b's shape and dtype, info 0 on convergence, else `maxiter`
+    (what scipy.sparse.linalg.gmres returns).  Follows scipy's restarted GMRES with `tol` as its rtol and
+    `num_krylov_vectors` as its restart: stops when ||b - A x|| <= max(atol, tol ||b||), atol=None meaning tol;
+    `maxiter` counts restart cycles, None meaning 10 b.size.  b = 0 gives x = 0, info 0.  An absent or zero x0 starts
+    from the residual b without a matvec; an x0 whose residual is already below the goal, or exactly 0 (where scipy
+    would divide by zero), is returned with info 0.  b and x0 are not modified.
+
+    Beyond the abstract method's checks (x0's shape: ValueError, x0's dtype: TypeError, tol or atol < 0 or
+    num_krylov_vectors <= 0 after clipping to b.size: ValueError):
+      - num_krylov_vectors=None means b.size; above 1024 after clipping it raises NotImplementedError;
+      - a preconditioner M raises NotImplementedError (only the numpy backend supports one);
+      - b must be float32/float64/complex64/complex128 (TypeError), maxiter >= 1 (ValueError);
+      - A_mv must return a `B200Tensor` (TypeError) of b's shape (ValueError); a complex result for a real b raises
+        TypeError.
+    An inner cycle ends early on breakdown, when the kernel finds the new Krylov vector in the span of the basis
+    (beta <= 16 sqrt(j + 2) eps ||w||, see tnb200_arnoldi_orth; scipy tests h1 <= eps h0), and the restarts end with
+    it.  The stopping test reads the Hessenberg column on the host at every step, so `jit` runs this eagerly."""
+    self._no_capture("gmres")        # (the Hessenberg column is read on the host at every step)
+    from . import gmres  # pylint: disable=import-outside-toplevel
+    return gmres.gmres(self, A_mv, b, A_args, A_kwargs, x0, tol, atol, num_krylov_vectors, maxiter, M)
+
 
 def register():
   """Insert the backend into the reference's registry (backend_factory.py:22-28)."""
