@@ -16,6 +16,9 @@ once into a *plan* (a flat list of backend calls) keyed by (shapes, labels, orde
 a cached plan is a straight loop of kernel launches with no Python list surgery, which is
 what makes CUDA-graph capture of a whole network possible (graph.py).
 """
+import ctypes
+import os
+
 import numpy as np
 from .tensor import B200Tensor
 
@@ -207,11 +210,9 @@ def execute_plan(backend, tensors, steps, result_slot):
   vals = list(tensors)
   for st in steps:
     op = st[0]
-    if op == "tensordot":
-      vals.append(backend.tensordot(vals[st[1]], vals[st[2]], (st[3], st[4])))
-    elif op == "batched":
-      vals.append(backend._contract(vals[st[1]], vals[st[2]], list(st[3]), list(st[4]),  # pylint: disable=protected-access
-                                    list(st[5]), list(st[6])))
+    if op in ("tensordot", "batched"):
+      ba, bb = _batch_axes(st)
+      vals.append(backend._contract(vals[st[1]], vals[st[2]], list(st[3]), list(st[4]), list(ba), list(bb)))  # pylint: disable=protected-access
     elif op == "ptrace":
       vals.append(backend.trace(backend.reshape(backend.transpose(vals[st[1]], st[2]), st[3])))
     elif op == "sum":
@@ -223,66 +224,10 @@ def execute_plan(backend, tensors, steps, result_slot):
   return vals[result_slot]
 
 
-def execute_plan_streams(backend, tensors, steps, result_slot, streams):
-  """Dependency-aware execution of a plan on several CUDA streams: every step runs on the stream
-  of its most recently produced operand and waits (event) only for operands produced elsewhere,
-  so independent branches of the contraction tree overlap.  Used under CUDA-graph capture, where
-  the stream/event structure becomes the graph's dependency edges.  Returns (result, all values)."""
-  torch = backend.torch
-  main = torch.cuda.current_stream()
-  vals = list(tensors)
-  home = [None] * len(vals)            # stream index that produced each slot (None: graph input)
-  events = {}
-  for s in streams:
-    s.wait_stream(main)
-  rr = 0
-  for st in steps:
-    op = st[0]
-    ins = [st[1], st[2]] if op in ("tensordot", "batched") else [st[1]]
-    out_slot = len(vals)
-    produced = [i for i in ins if home[i] is not None]
-    if op == "transpose":              # a view: no kernel, inherits its operand's stream
-      vals.append(backend.transpose(vals[st[1]], st[2]))
-      home.append(home[st[1]])
-      if st[1] in events:
-        events[out_slot] = events[st[1]]
-      continue
-    if not produced:
-      si = rr % len(streams)
-      rr += 1
-    else:
-      si = home[max(produced)]
-    stream = streams[si]
-    for i in produced:
-      if home[i] != si:
-        stream.wait_event(events[i])
-    with torch.cuda.stream(stream):
-      if op == "tensordot":
-        vals.append(backend.tensordot(vals[st[1]], vals[st[2]], (st[3], st[4])))
-      elif op == "batched":
-        vals.append(backend._contract(vals[st[1]], vals[st[2]], list(st[3]), list(st[4]),  # pylint: disable=protected-access
-                                      list(st[5]), list(st[6])))
-      elif op == "ptrace":
-        vals.append(backend.trace(backend.reshape(backend.transpose(vals[st[1]], st[2]), st[3])))
-      elif op == "sum":
-        vals.append(backend.sum(vals[st[1]], st[2]))
-      else:
-        raise RuntimeError("unknown plan step " + str(op))
-      e = torch.cuda.Event()
-      e.record(stream)
-      events[out_slot] = e
-    home.append(si)
-  for s in streams:
-    main.wait_stream(s)
-  return vals[result_slot], vals
-
-
 def ncon(tensors, network_structure, con_order=None, out_order=None, backend=None):
   """Same call signature / semantics as `tn.ncon` (ncon_interface.py:523) for backend tensors
   or numpy arrays (converted with `convert_to_tensor`, i.e. copied host->device)."""
-  if backend is None:
-    from .backend import get_instance  # pylint: disable=import-outside-toplevel
-    backend = get_instance()
+  backend = backend or _default()
   ts = [backend.convert_to_tensor(t) for t in tensors]
   shapes = tuple(t.shape for t in ts)
   key = ("ncon", shapes, _freeze(network_structure), _freeze(con_order), _freeze(out_order))
@@ -402,13 +347,11 @@ def plan_shapes(shapes, steps):
   shp = [tuple(s) for s in shapes]
   for st in steps:
     op = st[0]
-    if op == "tensordot":
+    if op in ("tensordot", "batched"):
       a, b = shp[st[1]], shp[st[2]]
-      out = [x for i, x in enumerate(a) if i not in st[3]] + [x for i, x in enumerate(b) if i not in st[4]]
-    elif op == "batched":
-      a, b = shp[st[1]], shp[st[2]]
-      ua, ub = set(st[3]) | set(st[5]), set(st[4]) | set(st[6])
-      out = [a[i] for i in st[5]] + [x for i, x in enumerate(a) if i not in ua] + [x for i, x in enumerate(b) if i not in ub]
+      ba, bb = _batch_axes(st)
+      ua, ub = set(st[3]) | set(ba), set(st[4]) | set(bb)
+      out = [a[i] for i in ba] + [x for i, x in enumerate(a) if i not in ua] + [x for i, x in enumerate(b) if i not in ub]
     elif op == "transpose":
       out = [shp[st[1]][p] for p in st[2]]
     else:
@@ -441,6 +384,40 @@ def _source(steps, n_inputs, slot):
   return slot
 
 
+def _inputs(st):
+  """the operand slots of a plan step"""
+  return (st[1], st[2]) if st[0] in ("tensordot", "batched") else (st[1],)
+
+
+def _batch_axes(st):
+  """the batch axes of a contraction step: a tensordot is a batched contraction without any"""
+  return st[5:7] if st[0] == "batched" else ((), ())
+
+
+def _contracted(st, shapes):
+  """the number of elements a contraction step sums over; `shapes` are the slot shapes of plan_shapes"""
+  return int(np.prod([shapes[st[1]][a] for a in st[3]] or [1]))
+
+
+def _users(steps):
+  """{slot: the steps that read it}, once per operand: a step that reads a slot twice is listed twice"""
+  users = {}
+  for i, st in enumerate(steps):
+    for x in _inputs(st):
+      users.setdefault(x, []).append(i)
+  return users
+
+
+def _linked_paths(nxt):
+  """the maximal paths s -> nxt[s] -> nxt[nxt[s]] ... of a successor map, in order of their first step"""
+  paths = []
+  for s in sorted(set(nxt) - set(nxt.values())):
+    paths.append([s])
+    while paths[-1][-1] in nxt:
+      paths[-1].append(nxt[paths[-1][-1]])
+  return paths
+
+
 def find_chain_groups(steps, n_inputs, res_slot, shapes):
   """Candidates for one chained launch each (tnb200_chain_create): lists of step indices in plan order.
 
@@ -456,19 +433,15 @@ def find_chain_groups(steps, n_inputs, res_slot, shapes):
   taken = {i for r in runs for i in r}
 
   def wide(i):
-    st = steps[i]
-    if i in taken or st[0] not in ("tensordot", "batched"):
-      return False
-    return int(np.prod([shapes[st[1]][a] for a in st[3]] or [1])) > 64
-  ins = [((st[1], st[2]) if st[0] != "transpose" else (st[1],)) for st in steps]
-  users = {}
-  for i, xs in enumerate(ins):
-    for x in xs:
+    return i not in taken and steps[i][0] in ("tensordot", "batched") and _contracted(steps[i], shapes) > 64
+  users = {}                                # consumers of each slot, looking through transposes
+  for i, st in enumerate(steps):
+    for x in _inputs(st):
       users.setdefault(_source(steps, n_inputs, x), set()).add(i)
   anc = []                                  # steps each step depends on, transitively
-  for i, xs in enumerate(ins):
+  for st in steps:
     a = set()
-    for x in xs:
+    for x in _inputs(st):
       p = _source(steps, n_inputs, x) - n_inputs
       if p >= 0:
         a |= anc[p] | {p}
@@ -479,23 +452,17 @@ def find_chain_groups(steps, n_inputs, res_slot, shapes):
     if wide(s) and n_inputs + s != res_slot and len(u) == 1 and wide(u[0]) and u[0] not in has_prev:
       nxt[s] = u[0]
       has_prev.add(u[0])
-  linked = []
-  for s in sorted(nxt):
-    if s not in has_prev:
-      linked.append([s])
-      while linked[-1][-1] in nxt:
-        linked[-1].append(nxt[linked[-1][-1]])
 
   def placeable(group):
     first, members = group[0], set(group)
     for i in group:
-      for x in ins[i]:
+      for x in _inputs(steps[i]):
         p = _source(steps, n_inputs, x) - n_inputs
         if p >= 0 and p not in members and p >= first:
           return False
     return True
   groups = []
-  for run in linked:
+  for run in _linked_paths(nxt):
     for k, g in enumerate(groups):
       if all(not (anc[i] & set(run)) for i in g) and all(not (anc[i] & set(g)) for i in run) \
           and placeable(sorted(g + run)):
@@ -514,15 +481,9 @@ def find_thin_runs(steps, n_inputs, res_slot, shapes, exclude=(), max_len=8):
   it is u's long operand (larger than u's other operand).  `shapes` are the slot shapes of plan_shapes; steps in
   `exclude` take no part.  Returns lists of at most `max_len` step indices, each at least two long."""
   def thin(i):
-    st = steps[i]
-    if i in exclude or st[0] not in ("tensordot", "batched"):
-      return False
-    return int(np.prod([shapes[st[1]][a] for a in st[3]] or [1])) <= 64
-  users = {}
-  for i, st in enumerate(steps):
-    for x in ((st[1], st[2]) if st[0] != "transpose" else (st[1],)):
-      users.setdefault(x, []).append(i)
-  nxt, has_prev = {}, set()
+    return i not in exclude and steps[i][0] in ("tensordot", "batched") and _contracted(steps[i], shapes) <= 64
+  users = _users(steps)
+  nxt = {}
   for s in range(len(steps)):
     out = n_inputs + s
     u = users.get(out, [])
@@ -531,14 +492,8 @@ def find_thin_runs(steps, n_inputs, res_slot, shapes, exclude=(), max_len=8):
     other = steps[u[0]][2] if steps[u[0]][1] == out else steps[u[0]][1]
     if other != out and np.prod(shapes[out]) > np.prod(shapes[other]):
       nxt[s] = u[0]
-      has_prev.add(u[0])
   runs = []
-  for s in sorted(nxt):
-    if s in has_prev:
-      continue
-    path = [s]
-    while path[-1] in nxt:
-      path.append(nxt[path[-1]])
+  for path in _linked_paths(nxt):
     runs += [path[i:i + max_len] for i in range(0, len(path), max_len) if len(path[i:i + max_len]) >= 2]
   return runs
 
@@ -575,7 +530,6 @@ class CompiledNetwork:
   def __init__(self, backend, shapes, dtype, labels, out_labels=(), path=None, nbatch=0,
                algorithm=None, num_streams=4, conj_aliases=None, use_chains=True):
     from . import tensor as T  # pylint: disable=import-outside-toplevel
-    from .tensor import B200Tensor  # pylint: disable=import-outside-toplevel
     self.backend = backend
     self.nbatch = nbatch
     torch = backend.torch
@@ -619,38 +573,25 @@ class CompiledNetwork:
       self.inputs.append(B200Tensor(view, code))
     self.num_pairwise = len(path)
     self.streams = [torch.cuda.Stream() for _ in range(max(1, num_streams))]
-    self._nodes = None
-    use_static = use_chains and all(st[0] in ("tensordot", "batched", "transpose") for st in self.steps)
-    if use_static:
-      self._build_static(code)
+    self._build_static(code, use_chains)
     # warm-up on a side stream (loads kernels, sets function attributes), then capture
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(side):
-      if self._nodes is not None:
-        self._run_nodes([side])
-      else:
-        execute_plan(backend, self.inputs, self.steps, self.res_slot)
+      self._run_nodes([side])
     torch.cuda.current_stream().wait_stream(side)
     torch.cuda.synchronize()
     self.graph = torch.cuda.CUDAGraph()
     l0 = backend.lib.tnb200_launch_count()
     with torch.cuda.graph(self.graph):
-      if self._nodes is not None:
-        self.output = self._run_nodes(self.streams)
-      elif num_streams > 1:
-        # keep every intermediate alive until capture ends: no buffer is recycled across streams
-        self.output, self._keep = execute_plan_streams(backend, self.inputs, self.steps, self.res_slot,
-                                                       self.streams)
-      else:
-        self.output = execute_plan(backend, self.inputs, self.steps, self.res_slot)
+      self.output = self._run_nodes(self.streams)
     self.launches_per_replay = int(backend.lib.tnb200_launch_count() - l0)
 
   # ------------------------------------------------------------------ static plan with chained launches
-  def _build_static(self, code):
+  def _build_static(self, code, use_chains):
     """Preallocate every step's result (addresses must be known before capture: chained launches freeze their
-    operand pointers at creation) and group the plan into nodes: single steps and chains."""
-    import ctypes  # pylint: disable=import-outside-toplevel
+    operand pointers at creation) and group the plan into nodes: single steps and chains.  Without `use_chains`
+    every contraction is a node of its own, writing its own buffer."""
     from . import _lib as L  # pylint: disable=import-outside-toplevel
     be = self.backend
     n_in = len(self.inputs)
@@ -658,16 +599,12 @@ class CompiledNetwork:
     # A result whose ONLY consumer is the next step of its run needs no buffer of its own: such results
     # alternate between two ring buffers (step s+2 starts, per sample, after step s+1 has consumed step s),
     # so a run's intermediates are overwritten while still dirty in L2 instead of being written back to HBM.
-    import os  # pylint: disable=import-outside-toplevel
     torch = be.torch
-    users = {}
-    for i, st in enumerate(self.steps):
-      for x in ((st[1], st[2]) if st[0] != "transpose" else (st[1],)):
-        users.setdefault(x, []).append(i)
     ring_of = {}
     nring = int(os.environ.get("TNB200_CHAIN_RING", "2"))
-    groups = find_chain_groups(self.steps, n_in, self.res_slot, shp)
+    groups = find_chain_groups(self.steps, n_in, self.res_slot, shp) if use_chains else []
     if nring >= 2:
+      users = _users(self.steps)
       # Ring slots are shared ONLY between results of identical shape (so sample b occupies the same region in
       # every step that uses the slot) and are handed out round-robin per shape: a slot written by step s is
       # next written by a step s' >= s + 2, which (per sample, through the run's read-after-write counters)
@@ -699,11 +636,6 @@ class CompiledNetwork:
     self._vals = vals
     chain_of = {}
     self.chains = []
-    pending = [list(g) for g in groups]
-    if code == L.F32 and be.math_mode in (L.MATH_STRICT, L.MATH_SIMT):
-      pending = []            # the chained kernel computes fp32 as TF32: strict fp32 stays on per-step launches
-    if be.math_mode == L.MATH_SIMT:
-      pending = []
     def step_array(run):
       pos = {sid: k for k, sid in enumerate(run)}
       arr = (L.ChainStep * len(run))()
@@ -712,10 +644,8 @@ class CompiledNetwork:
         a, b, c = vals[st[1]], vals[st[2]], vals[n_in + sid]
         cs = arr[k]
         cs.a, cs.b, cs.c = a.desc(), b.desc(), c.desc()
-        if st[0] == "tensordot":
-          ax_a, ax_b, ba, bb = st[3], st[4], (), ()
-        else:
-          ax_a, ax_b, ba, bb = st[3], st[4], st[5], st[6]
+        ax_a, ax_b = st[3], st[4]
+        ba, bb = _batch_axes(st)
         cs.naxes, cs.nbatch = len(ax_a), len(ba)
         for j, x in enumerate(ax_a):
           cs.axes_a[j] = x
@@ -725,9 +655,8 @@ class CompiledNetwork:
           cs.batch_a[j] = x
         for j, x in enumerate(bb):
           cs.batch_b[j] = x
-        # operands that are (views of) results of earlier steps of this run
-        cs.dep_a = self._producer(st[1], n_in, pos)
-        cs.dep_b = self._producer(st[2], n_in, pos)
+        # operands that are (views of) results of earlier steps of this run: their position in it, else -1
+        cs.dep_a, cs.dep_b = (pos.get(_source(self.steps, n_in, x) - n_in, -1) for x in _inputs(st))
       return arr
 
     def create(api, pending):
@@ -750,12 +679,14 @@ class CompiledNetwork:
           continue                                    # refused as a whole (too few tiles per step): step by step
         else:
           L.check(rc)
-    create("chain", pending)
-    # fused thin runs (16-bit only) among the steps no chain took; their intermediates stay on chip, so their
-    # buffers are released
-    thin_pending = [] if be.math_mode == L.MATH_SIMT else find_thin_runs(self.steps, n_in, self.res_slot, shp,
-                                                                         exclude=set(chain_of))
-    create("thin_run", thin_pending)
+    if use_chains:
+      # the chained kernel computes fp32 as TF32: strict fp32 stays on per-step launches
+      if not (be.math_mode == L.MATH_SIMT or (code == L.F32 and be.math_mode == L.MATH_STRICT)):
+        create("chain", [list(g) for g in groups])
+      # fused thin runs (16-bit only) among the steps no chain took; their intermediates stay on chip, so their
+      # buffers are released
+      if be.math_mode != L.MATH_SIMT:
+        create("thin_run", find_thin_runs(self.steps, n_in, self.res_slot, shp, exclude=set(chain_of)))
     for ch in self.chains:
       if ch.api == "thin_run":
         for sid in ch.steps[:-1]:
@@ -774,22 +705,14 @@ class CompiledNetwork:
         nodes.append((ch.api, ch))
     self._nodes = nodes
 
-  def _producer(self, slot, n_in, pos):
-    """position (inside the run `pos`) of the step that produced `slot`, looking through transposes; -1 if outside"""
-    slot = _source(self.steps, n_in, slot)
-    return pos.get(slot - n_in, -1) if slot >= n_in else -1
-
   def _node_io(self, node):
     n_in = len(self.inputs)
     if node[0] == "step":
-      st = self.steps[node[1]]
-      ins = [st[1], st[2]] if st[0] != "transpose" else [st[1]]
-      return ins, [n_in + node[1]]
+      return list(_inputs(self.steps[node[1]])), [n_in + node[1]]
     outs = [n_in + sid for sid in node[1].steps]
     ins = []
     for sid in node[1].steps:
-      st = self.steps[sid]
-      ins += [x for x in (st[1], st[2]) if x not in outs]
+      ins += [x for x in _inputs(self.steps[sid]) if x not in outs]
     if node[0] == "thin_run":
       outs = outs[-1:]                  # the run's intermediates never leave the chip
     return ins, outs
@@ -800,17 +723,17 @@ class CompiledNetwork:
       node[1].launch()
       return
     st = self.steps[node[1]]
-    if st[0] == "tensordot":
-      be._contract(vals[st[1]], vals[st[2]], list(st[3]), list(st[4]), [], [], out=vals[n_in + node[1]])  # pylint: disable=protected-access
-    elif st[0] == "batched":
-      be._contract(vals[st[1]], vals[st[2]], list(st[3]), list(st[4]), list(st[5]), list(st[6]),  # pylint: disable=protected-access
-                   out=vals[n_in + node[1]])
+    ba, bb = _batch_axes(st)
+    be._contract(vals[st[1]], vals[st[2]], list(st[3]), list(st[4]), list(ba), list(bb), out=vals[n_in + node[1]])  # pylint: disable=protected-access
 
   def _run_nodes(self, streams):
-    """dependency-aware execution of the node list on `streams` (the structure execute_plan_streams uses); all
-    chained launches share streams[0]: two persistent chain kernels must never wait for each other's SMs.  A node fed
-    only by chained launches takes the next stream in turn: the branches a chain leaves (the ramps after their heads)
-    then go on side by side instead of queueing behind one another on streams[0]."""
+    """Dependency-aware execution of the node list on `streams`: a node runs on the stream of its most recently
+    produced operand and waits (event) only for operands produced on other streams, so independent branches of the
+    contraction tree overlap; under CUDA-graph capture this stream/event structure becomes the graph's dependency
+    edges.  A transpose is a view and inherits its operand's stream.  All chained launches share streams[0]: two
+    persistent chain kernels must never wait for each other's SMs.  A node fed only by graph inputs or chained
+    launches takes the next stream in turn: the branches a chain leaves (the ramps after their heads) then go on side
+    by side instead of queueing behind one another on streams[0]."""
     torch = self.backend.torch
     main = torch.cuda.current_stream()
     multi = len(streams) > 1 or streams[0] is not main
@@ -860,9 +783,6 @@ class CompiledNetwork:
     static plan (a chained launch is one node).  `work` = (M, K, N) of every pairwise step in plan order.
     Bytes are algorithmic: operands + result of a step once; for a chain, only what enters and leaves the launch."""
     torch = self.backend.torch
-    if self._nodes is None:
-      raise RuntimeError("profile() needs the static plan (use_chains=True)")
-    n_in = len(self.inputs)
     cidx, k = {}, 0
     for i, st in enumerate(self.steps):
       if st[0] != "transpose":
@@ -947,9 +867,7 @@ def contract_network(tensors, labels, out_labels=(), path=None, backend=None,
                      algorithm=greedy_path, nbatch=0):
   """`contractors.greedy(nodes, output_edge_order)` on (tensor, labels) pairs: every label
   that appears on two tensors is a connected edge, labels in `out_labels` dangle."""
-  if backend is None:
-    from .backend import get_instance  # pylint: disable=import-outside-toplevel
-    backend = get_instance()
+  backend = backend or _default()
   ts = [backend.convert_to_tensor(t) for t in tensors]
   shapes = tuple(t.shape for t in ts)
   key = ("path", shapes, _freeze(labels), _freeze(out_labels), _freeze(path), nbatch)
