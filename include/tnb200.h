@@ -229,11 +229,33 @@ TNB200_API int32_t tnb200_qr(const tnb200_tensor_t* a, const tnb200_tensor_t* q,
 TNB200_API int32_t tnb200_lu_factor(const tnb200_tensor_t* a, const tnb200_tensor_t* lu, int32_t* piv_dev,
                                     int32_t* info_dev, void* stream);
 /* ---- NumPyBackend.inv (numpy_backend.py:554-558, np.linalg.inv): x = a^-1, x preallocated (n x n, any strides).
- *      The factorisation above, then a blocked solve against the permuted identity (forward with unit L, backward with
- *      U, 32 rows per step: a triangular solve and one update launch each, the update on DMMA for f64).  Launches:
+ *      The factorisation above, then tnb200_lu_solve's blocked solve against the identity (the row interchanges, then
+ *      forward with unit L and backward with U, 32 rows per step: a triangular solve and one update launch each, the
+ *      update on DMMA for f64).  Launches:
  *      at most 8 ceil(n / 32) + 8.  info_dev[0] as for tnb200_lu_factor: nonzero means the matrix is singular and x
  *      holds no inverse.  Same dtypes and errors as tnb200_lu_factor.  Does not synchronise with the host. */
 TNB200_API int32_t tnb200_inv(const tnb200_tensor_t* a, const tnb200_tensor_t* x, int32_t* info_dev, void* stream);
+/* ---- LAPACK getrs / scipy.linalg.lu_solve on tnb200_lu_factor's output: x = a^-1 b with lu (n x n) and piv_dev[n] as
+ *      lu_factor wrote them; b and x are n x k, any strides (x may not overlap b).  The row interchanges on b, then the
+ *      blocked forward (unit L) and backward (U) substitution of tnb200_inv, 32 rows per step.  Same dtypes, widening
+ *      and errors as tnb200_lu_factor; all three of one dtype.  n = 0 or k = 0: no-op.  Does not synchronise with the
+ *      host. */
+TNB200_API int32_t tnb200_lu_solve(const tnb200_tensor_t* lu, const int32_t* piv_dev, const tnb200_tensor_t* b,
+                                   const tnb200_tensor_t* x, void* stream);
+
+/* ---- NumPyBackend.expm (numpy_backend.py:589-598, scipy.linalg.expm): x = exp(a) for the n x n view `a`, x
+ *      preallocated n x n, any strides.  Scaling and squaring with Pade degrees 3, 5, 7, 9, 13 (Al-Mohy & Higham 2009,
+ *      Algorithm 5.1) and the degree / squaring choice of scipy.sparse.linalg._matfuncs._expm with exact 1-norms.  f32 /
+ *      c64 are widened to f64 / c128 and rounded back.  Any NaN or Inf in `a` gives an all-NaN x, as scipy returns.
+ *      info_dev (device int32[4], may be NULL) receives {m, s, path, lu_info}: the Pade degree, the number of squarings,
+ *      0 for the fused path or 1 for the blocked one, and the getrf info of the Q factorisation.
+ *        - n <= TNB200_EXPM_FUSED_MAX_N: ONE launch, one CTA, no host synchronisation (capturable);
+ *        - larger n: GEMMs through tnb200_tensordot's dispatch in strict mode (DMMA for f64), Q factored and solved as
+ *          in tnb200_inv; the host reads the selection at most three times (once per stage that decides which power
+ *          of a to form next).
+ *      Other dtypes: TNB200_ERR_DTYPE; not square: TNB200_ERR_INVALID; n = 0: no-op. */
+#define TNB200_EXPM_FUSED_MAX_N 48
+TNB200_API int32_t tnb200_expm(const tnb200_tensor_t* a, const tnb200_tensor_t* x, int32_t* info_dev, void* stream);
 
 /* ---- a11: block_sparse.tensordot per-sector loop (block_sparse/blocksparsetensor.py:1094-1101).
  * For each sector q: C.data[c_map[q]] = A.data[a_map[q]].reshape(m_q,k_q) @ B.data[b_map[q]]

@@ -21,6 +21,8 @@ CONJ, SQRT, ABS, NEG, EXP, LOG, SIN, COS, SIGN, REAL, IMAG = range(11)
 LT, LE, GT, GE = range(4)
 CONJ_A, CONJ_B = 1, 2
 MATH_DEFAULT, MATH_STRICT, MATH_SIMT = 0 << 4, 1 << 4, 2 << 4
+# TNB200_EXPM_FUSED_MAX_N: tnb200_expm runs in one launch without host reads up to this n
+EXPM_FUSED_MAX_N = 48
 
 
 class TensorDesc(ctypes.Structure):
@@ -73,6 +75,8 @@ SIGNATURES = {
     "tnb200_qr": (_i32, [_P, _P, _P, _i32, _vp]),
     "tnb200_lu_factor": (_i32, [_P, _P, _vp, _vp, _vp]),
     "tnb200_inv": (_i32, [_P, _P, _vp, _vp]),
+    "tnb200_lu_solve": (_i32, [_P, _vp, _P, _P, _vp]),
+    "tnb200_expm": (_i32, [_P, _P, _vp, _vp]),
     "tnb200_blocksparse_maps": (_i32, [_i32, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _i64, _i32, _vp, _i64, _vp, _vp]),
     "tnb200_svd_batched": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "tnb200_gather": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp]),

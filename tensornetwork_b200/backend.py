@@ -755,6 +755,39 @@ class CudaB200Backend(_Base):
       raise np.linalg.LinAlgError("Singular matrix")
     return x
 
+  # result dtype of expm per input dtype, as scipy.linalg.expm returns it (bf16 is treated like f16)
+  _EXPM_CODE = {L.F64: L.F64, L.F32: L.F32, L.C64: L.C64, L.C128: L.C128, L.I32: L.F64, L.I64: L.F64, L.BOOL: L.F64,
+                L.F16: L.F32, L.BF16: L.F32}
+
+  def expm(self, matrix):
+    """numpy_backend.py:589-598 (scipy.linalg.expm): scaling and squaring with Pade approximants (tnb200_expm), the
+    degree and squaring count chosen as scipy's `_expm` chooses them with exact 1-norms.  Integer and bool input
+    gives float64, f16 / bf16 give float32; a NaN or Inf entry gives an all-NaN result.  0 x 0 returns an empty
+    tensor of the input dtype and 1 x 1 the elementwise exp, as scipy does.  Up to `_lib.EXPM_FUSED_MAX_N` the call is
+    one launch with no host read, so `jit` captures it; above, the kernel reads its degree selection on the host and
+    `jit` runs it eagerly."""
+    self._check_type(matrix)
+    if matrix.ndim != 2:
+      raise ValueError("input to numpy backend method `expm` has shape {}."
+                       " Only matrices are supported.".format(matrix.shape))
+    n, m = matrix.shape
+    if n != m:
+      raise ValueError("input to numpy backend method `expm` only supports"
+                       " N*N matrix, {x}*{y} matrix is given".format(x=n, y=m))
+    if n == 0:
+      return self._new((0, 0), matrix.code)
+    if n > L.EXPM_FUSED_MAX_N:
+      self._no_capture("expm")       # (the degree selection is read on the host)
+    if matrix.code == L.BOOL:        # (the copy kernels take no bool): 1.0 where the mask is set
+      matrix = self.index_update(self.zeros((n, n), np.float64), matrix, 1.0)
+    matrix = self.astype(matrix, self._EXPM_CODE[matrix.code])
+    if n == 1:
+      return self.exp(matrix)
+    x = self._new((n, n), matrix.code)
+    info = self.torch.empty(4, dtype=self.torch.int32, device=self.device)
+    L.check(self.lib.tnb200_expm(matrix.ref(), x.ref(), info.data_ptr(), self._stream()))
+    return x
+
   def rq(self, tensor, pivot_axis=-1, non_negative_diagonal=False):
     """decompositions.py:101-124: QR of the conjugate transpose, then conjugate back."""
     self._check_type(tensor)

@@ -40,6 +40,18 @@ __device__ __forceinline__ zd unit_conj_phase(zd g) {
 
 __device__ __forceinline__ zd divz(zd a, zd b) { double d = b.x * b.x + b.y * b.y; return zd{(a.x * b.x + a.y * b.y) / d, (a.y * b.x - a.x * b.y) / d}; }
 __device__ __forceinline__ double divz(double a, double b) { return a / b; }
+__device__ __forceinline__ double pivmag(double a) { return fabs(a); }
+__device__ __forceinline__ double pivmag(zd a) { return fabs(a.x) + fabs(a.y); }   // dcabs1, as izamax ranks
+// a / b without forming |b|^2 (Smith's algorithm): no overflow or underflow for |b| anywhere in the double range
+__device__ __forceinline__ double divs(double a, double b) { return a / b; }
+__device__ __forceinline__ zd divs(zd a, zd b) {
+  if (fabs(b.x) >= fabs(b.y)) {
+    const double r = b.y / b.x, d = b.x + b.y * r;
+    return zd{(a.x + a.y * r) / d, (a.y - a.x * r) / d};
+  }
+  const double r = b.x / b.y, d = b.x * r + b.y;
+  return zd{(a.x * r + a.y) / d, (a.y * r - a.x) / d};
+}
 __device__ __forceinline__ double im_(double) { return 0.0; }
 __device__ __forceinline__ double im_(zd a) { return a.y; }
 __device__ __forceinline__ double mk(double re, double, double*) { return re; }

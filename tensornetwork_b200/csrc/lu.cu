@@ -1,5 +1,6 @@
-// lu.cu — tnb200_lu_factor / tnb200_inv: LU with partial pivoting (LAPACK getrf, the pivots scipy.linalg.lu_factor
-// returns) and the inverse built on it (np.linalg.inv, NumPyBackend.inv, backends/numpy/numpy_backend.py:554-558).
+// lu.cu — tnb200_lu_factor / tnb200_lu_solve / tnb200_inv: LU with partial pivoting (LAPACK getrf, the pivots
+// scipy.linalg.lu_factor returns), the solve on its factors (getrs, scipy.linalg.lu_solve) and the inverse built on both
+// (np.linalg.inv, NumPyBackend.inv, backends/numpy/numpy_backend.py:554-558).
 //
 // Working storage is column-major (W[c * n + r]) in double or zd; f32 / c64 are widened by the strided copy in and
 // rounded back by the copy out.  Right-looking blocked LU, panels of LB = 32 columns, four launches per panel:
@@ -12,8 +13,9 @@
 //   lu_laswp_kernel  : the panel's interchanges on the columns left and right of it (one thread per column).
 //   lu_trsm_kernel   : U12 = L11^-1 A12 (unit lower, 32 x 32 in shared memory, one thread per column).
 //   lu_update_*      : A22 -= L21 U12 — DMMA m8n8k4 for f64, CUDA-core FMA for c128.
-// The inverse solves A X = I as X = U^-1 (L^-1 (P I)): the permuted identity is written directly, then forward and
-// backward block substitution, 32 rows per step, each step one triangular-solve launch and one update launch.
+// The solve (lu_solve_ws, shared with expm.cu) computes X = U^-1 (L^-1 (P B)): the row interchanges on B, then forward and
+// backward block substitution, 32 rows per step, each step one triangular-solve launch and one update launch.  The
+// inverse is the solve with B = I.
 #include "common.cuh"
 #include "cplx.cuh"
 #include <float.h>
@@ -25,18 +27,6 @@ int copy_strided(const tnb200_tensor_t* src, const tnb200_tensor_t* dst, int con
 
 constexpr int LB = 32, LCL = 8, LTHR = 256;
 
-__device__ __forceinline__ double pivmag(double a) { return fabs(a); }
-__device__ __forceinline__ double pivmag(zd a) { return fabs(a.x) + fabs(a.y); }   // dcabs1, as izamax ranks
-// a / b without forming |b|^2 (Smith's algorithm): no overflow or underflow for |b| anywhere in the double range
-__device__ __forceinline__ double divs(double a, double b) { return a / b; }
-__device__ __forceinline__ zd divs(zd a, zd b) {
-  if (fabs(b.x) >= fabs(b.y)) {
-    const double r = b.y / b.x, d = b.x + b.y * r;
-    return zd{(a.x + a.y * r) / d, (a.y - a.x * r) / d};
-  }
-  const double r = b.x / b.y, d = b.x * r + b.y;
-  return zd{(a.x * r + a.y) / d, (a.y * r - a.x) / d};
-}
 __device__ __forceinline__ bool is_zero(double a) { return a == 0.0; }
 __device__ __forceinline__ bool is_zero(zd a) { return a.x == 0.0 && a.y == 0.0; }
 
@@ -324,28 +314,16 @@ static void lu_update(const LuUpd<zd>& u, cudaStream_t st) {
   lu_update_fma_kernel<zd><<<dim3((unsigned)((u.M + 63) / 64), (unsigned)((u.N + 63) / 64)), 256, 0, st>>>(u);
 }
 
-// X = P I: row i of P A is row perm[i] of A, so X[i, perm[i]] = 1.  perm is built from piv by one thread, in shared
-// memory when it fits (the swaps are a dependent chain), otherwise in place in global memory.
-__global__ void lu_perm_kernel(const int* __restrict__ piv, int* __restrict__ perm, int n, int in_smem) {
-  extern __shared__ int psm[];
-  int* p = in_smem ? psm : perm;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) p[i] = i;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int k = 0; k < n; ++k) {
-      const int r = piv[k];
-      const int t = p[k]; p[k] = p[r]; p[r] = t;
-    }
-  }
-  __syncthreads();
-  if (in_smem)
-    for (int i = threadIdx.x; i < n; i += blockDim.x) perm[i] = p[i];
-}
+// B <- P B: the interchanges piv[0..n) of the factorisation applied in order to each of the nrhs columns of B (LAPACK's
+// laswp on the right-hand side), one thread per column
 template <typename T>
-__global__ void lu_perm_eye_kernel(const int* __restrict__ perm, T* __restrict__ X, int64_t n) {
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < n * n; idx += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t c = idx / n, r = idx - c * n;
-    X[idx] = perm[r] == c ? one_<T>() : zero_<T>();
+__global__ void lu_laswp_rhs_kernel(T* __restrict__ B, int64_t ldb, int64_t n, int64_t nrhs, const int* __restrict__ piv) {
+  const int64_t col = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (col >= nrhs) return;
+  T* x = B + col * ldb;
+  for (int64_t k = 0; k < n; ++k) {
+    const int r = piv[k];
+    if (r != k) { const T v = x[k]; x[k] = x[r]; x[r] = v; }
   }
 }
 
@@ -357,7 +335,7 @@ static unsigned lu_grid(int64_t work, int threads) {
 
 // LU of W (n x n, column-major, in place); piv / info device arrays, info[0] must be 0 on entry
 template <typename T>
-static int lu_factor_ws(T* W, int64_t n, int* piv, int* info, cudaStream_t st, int* launches) {
+int lu_factor_ws(T* W, int64_t n, int* piv, int* info, cudaStream_t st, int* launches) {
   static bool attr_done = false;
   if (!attr_done) {
     TNB_CHECK_CUDA(cudaFuncSetAttribute(lu_panel_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024));
@@ -386,37 +364,29 @@ static int lu_factor_ws(T* W, int64_t n, int* piv, int* info, cudaStream_t st, i
   return 0;
 }
 
-// X = A^-1 from the factors in W: X = P I, then forward (unit L) and backward (U) block substitution
+// B <- A^-1 B (LAPACK getrs) from the factors in W: the row interchanges, then forward (unit L) and backward (U) block
+// substitution, 32 rows per step.  B is n x nrhs, column-major with leading dimension ldb.
 template <typename T>
-static int lu_inverse_ws(const T* W, int64_t n, const int* piv, int* perm, T* X, cudaStream_t st, int* launches) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    TNB_CHECK_CUDA(cudaFuncSetAttribute(lu_perm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_done = true;
-  }
-  const bool in_smem = sizeof(int) * (size_t)n <= 200 * 1024;
-  lu_perm_kernel<<<1, 256, in_smem ? sizeof(int) * (size_t)n : 0, st>>>(piv, perm, (int)n, in_smem ? 1 : 0);
-  int64_t blocks = (n * n + 255) / 256;
-  if (blocks > (int64_t)num_sms() * 16) blocks = (int64_t)num_sms() * 16;
-  lu_perm_eye_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(perm, X, n);
-  *launches += 2;
+int lu_solve_ws(const T* W, int64_t n, const int* piv, T* B, int64_t ldb, int64_t nrhs, cudaStream_t st, int* launches) {
+  lu_laswp_rhs_kernel<T><<<lu_grid(nrhs, 128), 128, 0, st>>>(B, ldb, n, nrhs, piv);
+  ++*launches;
   for (int64_t r0 = 0; r0 < n; r0 += LB) {
     const int b = (int)(n - r0 < LB ? n - r0 : LB);
-    lu_trsm_kernel<T><<<lu_grid(n, 128), 128, 0, st>>>(W, n, (int)r0, b, 0, X, n, 0, n);
+    lu_trsm_kernel<T><<<lu_grid(nrhs, 128), 128, 0, st>>>(W, n, (int)r0, b, 0, B, ldb, 0, nrhs);
     ++*launches;
     const int64_t below = n - r0 - b;
     if (below > 0) {
-      LuUpd<T> u{W + r0 * n + r0 + b, n, X + r0, n, X + r0 + b, n, below, n, b};
+      LuUpd<T> u{W + r0 * n + r0 + b, n, B + r0, ldb, B + r0 + b, ldb, below, nrhs, b};
       lu_update(u, st);
       ++*launches;
     }
   }
   for (int64_t r0 = ((n - 1) / LB) * LB; r0 >= 0; r0 -= LB) {
     const int b = (int)(n - r0 < LB ? n - r0 : LB);
-    lu_trsm_kernel<T><<<lu_grid(n, 128), 128, 0, st>>>(W, n, (int)r0, b, 1, X, n, 0, n);
+    lu_trsm_kernel<T><<<lu_grid(nrhs, 128), 128, 0, st>>>(W, n, (int)r0, b, 1, B, ldb, 0, nrhs);
     ++*launches;
     if (r0 > 0) {
-      LuUpd<T> u{W + r0 * n, n, X + r0, n, X, n, r0, n, b};
+      LuUpd<T> u{W + r0 * n, n, B + r0, ldb, B, ldb, r0, nrhs, b};
       lu_update(u, st);
       ++*launches;
     }
@@ -424,6 +394,10 @@ static int lu_inverse_ws(const T* W, int64_t n, const int* piv, int* perm, T* X,
   TNB_LAUNCH_CHECK();
   return 0;
 }
+template int lu_factor_ws<double>(double*, int64_t, int*, int*, cudaStream_t, int*);
+template int lu_factor_ws<zd>(zd*, int64_t, int*, int*, cudaStream_t, int*);
+template int lu_solve_ws<double>(const double*, int64_t, const int*, double*, int64_t, int64_t, cudaStream_t, int*);
+template int lu_solve_ws<zd>(const zd*, int64_t, const int*, zd*, int64_t, int64_t, cudaStream_t, int*);
 
 static tnb200_tensor_t colmajor(void* p, int dtype, int64_t n) {
   tnb200_tensor_t t;
@@ -459,15 +433,14 @@ static int lu_run(const tnb200_tensor_t* a, const tnb200_tensor_t* lu, const tnb
   rc = copy_strided(a, &tw, 0, st);
   if (rc == 0) rc = lu_factor_ws<T>(W, n, piv, info, st, &launches);
   if (rc == 0 && lu) rc = copy_strided(&tw, lu, 0, st);
-  if (rc == 0 && x) {
+  if (rc == 0 && x) {                              // A X = I: the solve with B = I
     T* X = nullptr;
-    int* perm = nullptr;
     rc = ws_alloc((void**)&X, sizeof(T) * (size_t)n * n, st);
-    if (rc == 0) rc = ws_alloc((void**)&perm, sizeof(int) * (size_t)n, st);
-    if (rc == 0) rc = lu_inverse_ws<T>(W, n, piv, perm, X, st, &launches);
     tnb200_tensor_t tx = colmajor(X, wide, n);
+    if (rc == 0) rc = tnb200_eye(&tx, 0, st);
+    if (rc == 0) rc = lu_solve_ws<T>(W, n, piv, X, n, n, st, &launches);
     if (rc == 0) rc = copy_strided(&tx, x, 0, st);
-    ws_free(X, st); ws_free(perm, st);             // (ws_free ignores NULL)
+    ws_free(X, st);                                // (ws_free ignores NULL)
   }
   count_launch(launches);
   ws_free(W, st);
@@ -489,6 +462,43 @@ extern "C" int32_t tnb200_lu_factor(const tnb200_tensor_t* a, const tnb200_tenso
   set_kernel_name(a->dtype == TNB200_F64 || a->dtype == TNB200_F32 ? "lu_blocked_dmma" : "lu_blocked_fma");
   if (dtype_is_complex(a->dtype)) return lu_run<zd>(a, lu, nullptr, piv_dev, info_dev, st);
   return lu_run<double>(a, lu, nullptr, piv_dev, info_dev, st);
+}
+
+extern "C" int32_t tnb200_lu_solve(const tnb200_tensor_t* lu, const int32_t* piv_dev, const tnb200_tensor_t* b,
+                                   const tnb200_tensor_t* x, void* stream) {
+  TNB_REQUIRE(valid_tensor(lu) && valid_tensor(b) && valid_tensor(x), TNB200_ERR_INVALID, "lu_solve: invalid tensor descriptor");
+  TNB_REQUIRE(lu->ndim == 2 && b->ndim == 2 && x->ndim == 2, TNB200_ERR_INVALID, "lu_solve: expects matrices");
+  TNB_REQUIRE(lu->shape[0] == lu->shape[1], TNB200_ERR_INVALID, "lu_solve: the factors must be square, got %lld x %lld",
+              (long long)lu->shape[0], (long long)lu->shape[1]);
+  TNB_REQUIRE(b->shape[0] == lu->shape[0], TNB200_ERR_INVALID, "lu_solve: b has %lld rows, the factors %lld",
+              (long long)b->shape[0], (long long)lu->shape[0]);
+  TNB_REQUIRE(x->shape[0] == b->shape[0] && x->shape[1] == b->shape[1], TNB200_ERR_INVALID, "lu_solve: x must have b's shape");
+  TNB_REQUIRE(b->dtype == lu->dtype && x->dtype == lu->dtype, TNB200_ERR_DTYPE, "lu_solve: dtype mismatch");
+  TNB_REQUIRE(lu->dtype == TNB200_F64 || lu->dtype == TNB200_F32 || lu->dtype == TNB200_C128 || lu->dtype == TNB200_C64,
+              TNB200_ERR_DTYPE, "lu_solve: dtype %s is not supported (f32/f64/c64/c128)", dtype_name(lu->dtype));
+  TNB_REQUIRE(lu->shape[0] < (1LL << 31), TNB200_ERR_UNSUPPORTED, "lu_solve: matrix too large");
+  const int64_t n = lu->shape[0], k = b->shape[1];
+  if (n == 0 || k == 0) return 0;
+  TNB_REQUIRE(piv_dev, TNB200_ERR_INVALID, "lu_solve: piv must be a device array");
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool cplx = dtype_is_complex(lu->dtype);
+  const int wide = cplx ? TNB200_C128 : TNB200_F64;
+  const size_t es = cplx ? 16 : 8;
+  set_kernel_name(cplx ? "lu_solve_fma" : "lu_solve_dmma");
+  void *W = nullptr, *X = nullptr;
+  int rc = ws_alloc(&W, es * (size_t)n * n, st);
+  if (rc == 0) rc = ws_alloc(&X, es * (size_t)n * k, st);
+  tnb200_tensor_t tw = colmajor(W, wide, n), tx = colmajor(X, wide, n);
+  tx.shape[1] = k;
+  int launches = 0;
+  if (rc == 0) rc = copy_strided(lu, &tw, 0, st);
+  if (rc == 0) rc = copy_strided(b, &tx, 0, st);
+  if (rc == 0) rc = cplx ? lu_solve_ws<zd>((const zd*)W, n, piv_dev, (zd*)X, n, k, st, &launches)
+                         : lu_solve_ws<double>((const double*)W, n, piv_dev, (double*)X, n, k, st, &launches);
+  if (rc == 0) rc = copy_strided(&tx, x, 0, st);
+  count_launch(launches);
+  ws_free(W, st); ws_free(X, st);
+  return rc;
 }
 
 extern "C" int32_t tnb200_inv(const tnb200_tensor_t* a, const tnb200_tensor_t* x, int32_t* info_dev, void* stream) {
