@@ -280,6 +280,25 @@ TNB200_API int32_t tnb200_svd_batched(const void* a_data, int32_t dtype, int32_t
                                       const int64_t* s_off_dev, void* vh_data, const int64_t* vh_off_dev,
                                       int64_t max_m, int64_t max_n, int32_t* status_dev, void* stream);
 
+/* ---- the per-sector QRs of block_sparse/linalg.py:300-393 (a Python loop of np.linalg.qr there): `nprob` independent
+ * reduced Householder QRs in ONE launch, one CTA per matrix, staged column-major in shared memory (f32 / c64 widened
+ * to f64 / c128).  Problem q: A_q is m_q x n_q, row-major contiguous at a_data + a_off[q] (element offsets); dims holds
+ * (m_q, n_q) pairs; r = min(m, n).  The reflectors are tnb200_qr's (LAPACK geqrf + orgqr: beta = -sign(Re alpha) |x|),
+ * so each Q_q, R_q is np.linalg.qr(A_q) to rounding.  Outputs are row-major at the given offsets:
+ *   adjoint = 0:  Q_q (m x r) and R_q (r x n, upper trapezoidal with explicit zeros): A_q = Q_q R_q;
+ *   adjoint = 1:  the factors of A_q^H = Q' R', written as R_q = R'^H (m x r) and Q_q = Q'^H (r x n): A_q = R_q Q_q,
+ *                 the block-sparse RQ of backends/symmetric/decompositions.py:234-248.
+ * max_elems bounds m_q n_q over all problems and sizes the shared memory: sizeof(f64 or c128) * max_elems must not
+ * exceed TNB200_QR_BATCHED_MAX_BYTES (TNB200_ERR_UNSUPPORTED; use tnb200_qr for such a problem).  A problem with
+ * m_q n_q > max_elems is skipped.  All arrays are device pointers; nprob = 0 and empty problems are no-ops; no host
+ * synchronisation.  Bad sizes or null pointers: TNB200_ERR_INVALID; dtypes other than f64 / f32 / c128 / c64:
+ * TNB200_ERR_DTYPE.  The limit is what fits in shared memory, not a measured crossover (README: one problem alone beats
+ * tnb200_qr up to n = 64 in f64 and n = 112 in c128 on an H100 80GB HBM3 at 700 W; a batch runs its problems at once). */
+#define TNB200_QR_BATCHED_MAX_BYTES (200 * 1024)
+TNB200_API int32_t tnb200_qr_batched(const void* a_data, int32_t dtype, int32_t nprob, const int64_t* dims_dev,
+                                     const int64_t* a_off_dev, void* q_data, const int64_t* q_off_dev, void* r_data,
+                                     const int64_t* r_off_dev, int64_t max_elems, int32_t adjoint, void* stream);
+
 /* ---- f3: the int64 element maps of a block-sparse matrix view, built on the device (the reference builds them on the host
  * with numpy unique / intersect: block_sparse/blocksparse_utils.py:330-634, cached only on request, caching.py:22-88).
  * The tensor has `nlegs` stored legs; leg t has dims[t] states with SIGNED charges (flow applied, int64) at

@@ -23,6 +23,8 @@ CONJ_A, CONJ_B = 1, 2
 MATH_DEFAULT, MATH_STRICT, MATH_SIMT = 0 << 4, 1 << 4, 2 << 4
 # TNB200_EXPM_FUSED_MAX_N: tnb200_expm runs in one launch without host reads up to this n
 EXPM_FUSED_MAX_N = 48
+# TNB200_QR_BATCHED_MAX_BYTES: tnb200_qr_batched takes problems with sizeof(f64 or c128) * m * n up to this
+QR_BATCHED_MAX_BYTES = 200 * 1024
 
 
 class TensorDesc(ctypes.Structure):
@@ -79,6 +81,7 @@ SIGNATURES = {
     "tnb200_expm": (_i32, [_P, _P, _vp, _vp]),
     "tnb200_blocksparse_maps": (_i32, [_i32, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _i64, _i32, _vp, _i64, _vp, _vp]),
     "tnb200_svd_batched": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
+    "tnb200_qr_batched": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp]),
     "tnb200_gather": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp]),
     "tnb200_blocksparse_tensordot": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
                                             _vp, _vp, _i64, _i64, _i32, _vp]),

@@ -492,6 +492,67 @@ def _truncate_sectors(singvals, max_singular_values=None, max_truncation_error=N
   return kept, discarded
 
 
+def _pack_sectors(tensor, nl):
+  """The charge sectors of the matrix view (legs order[:nl] | order[nl:]) packed row-major, sector after sector, into one
+  device buffer by one `tnb200_gather`.  Returns (qnums, ms, ns, a_off (nsect + 1 element offsets), buffer)."""
+  be = tensor.backend
+  qn, dims, maps = _sector_maps(tensor.indices, tensor.order, nl)
+  ms, ns = dims[:, 0], dims[:, 1]
+  a_off = np.zeros(len(maps) + 1, dtype=np.int64); a_off[1:] = np.cumsum(ms * ns)
+  a_buf = be._new((int(a_off[-1]),), tensor.data.code)  # pylint: disable=protected-access
+  gmap = _up(be, np.concatenate(maps) if maps else np.zeros(0, dtype=np.int64))
+  L.check(be.lib.tnb200_gather(tensor.data.t.data_ptr(), gmap.data_ptr(), a_buf.t.data_ptr(), int(a_off[-1]), tensor.data.code, 0,
+                               be._stream()))  # pylint: disable=protected-access
+  return qn, ms, ns, a_off, a_buf
+
+
+def _up(be, x):
+  return be.torch.from_numpy(np.ascontiguousarray(x, dtype=np.int64)).to(be.device)
+
+
+def _take(be, buf, idx, code):
+  """buf[idx] as a new device vector (one `tnb200_gather`)."""
+  out = be._new((len(idx),), code)  # pylint: disable=protected-access
+  if len(idx):
+    L.check(be.lib.tnb200_gather(buf.t.data_ptr(), _up(be, idx).data_ptr(), out.t.data_ptr(), len(idx), code, 0,
+                                 be._stream()))  # pylint: disable=protected-access
+  return out
+
+
+def _cat(xs):
+  return np.concatenate(xs) if xs else np.zeros(0, dtype=np.int64)
+
+
+def _factor_tensors(tensor, nl, qn, ms, ns, kept, l_buf, l_off, r_buf, r_off):
+  """The block-sparse factors of a per-sector decomposition A_q = L_q R_q with L_q (m x r) and R_q (r x n), r = min(m, n),
+  row-major at l_off[q] / r_off[q] of the packed buffers, keeping the first kept[q] columns of L_q and rows of R_q.
+
+  Returns (L, R): L legs = left legs + [bond], bond flow True; R legs = [bond] + right legs, bond flow False
+  (block_sparse/linalg.py:343-392).  The bond carries the sector charge kept[q] times, sector-major."""
+  be, code = tensor.backend, tensor.data.code
+  l_idx, r_idx, bond_q = [], [], []
+  for q, k in enumerate(kept):
+    if k == 0:
+      continue
+    m_, n_, r_ = int(ms[q]), int(ns[q]), int(min(ms[q], ns[q]))
+    b = np.arange(k)
+    l_idx.append((l_off[q] + np.arange(m_)[None, :] * r_ + b[:, None]).ravel())      # (k x m): l_q[:, :k].T
+    r_idx.append((r_off[q] + b[:, None] * n_ + np.arange(n_)[None, :]).ravel())      # (k x n): r_q[:k, :]
+    bond_q.append(np.full(k, qn[q], dtype=np.int64))
+  l_data = _take(be, l_buf, _cat(l_idx), code)
+  r_data = _take(be, r_buf, _cat(r_idx), code)
+  mod = tensor.indices[0].modulus if tensor.indices else None
+  bond_charges = _cat(bond_q)
+  left = [tensor.indices[tensor.order[i]] for i in range(nl)]
+  right = [tensor.indices[tensor.order[i]] for i in range(nl, tensor.ndim)]
+  bond_l = Index(bond_charges, True, mod)
+  bond_r = Index(bond_charges, False, mod)
+  Lt = BlockSparseTensor(l_data, [bond_l] + left, list(range(1, nl + 1)) + [0], be)
+  Rt = BlockSparseTensor(r_data, [bond_r] + right, None, be)
+  assert l_data.size == BlockSparseTensor._nnz([bond_l] + left) and r_data.size == BlockSparseTensor._nnz([bond_r] + right)  # pylint: disable=protected-access
+  return Lt, Rt
+
+
 def svd(tensor, pivot_axis, max_singular_values=None, max_truncation_error=None, relative=False):
   """Block-sparse SVD (backends/symmetric/decompositions.py:27-216): one small SVD per charge sector —
   all sectors in ONE `tnb200_svd_batched` launch — then the reference's global truncation.
@@ -502,26 +563,21 @@ def svd(tensor, pivot_axis, max_singular_values=None, max_truncation_error=None,
   be = tensor.backend
   torch = be.torch
   nl = pivot_axis if pivot_axis >= 0 else tensor.ndim + pivot_axis
-  qn, dims, maps = _sector_maps(tensor.indices, tensor.order, nl)
   code = tensor.data.code
   if code not in (L.F64, L.F32, L.C64, L.C128):
     raise TypeError("block-sparse svd needs a float32/float64/complex tensor")
-  nsect = len(maps)
-  ms, ns = dims[:, 0], dims[:, 1]
+  qn, ms, ns, a_off, a_buf = _pack_sectors(tensor, nl)
+  nsect = len(qn)
   rs = np.minimum(ms, ns)
-  a_off = np.zeros(nsect + 1, dtype=np.int64); a_off[1:] = np.cumsum(ms * ns)
   u_off = np.zeros(nsect + 1, dtype=np.int64); u_off[1:] = np.cumsum(ms * rs)
   s_off = np.zeros(nsect + 1, dtype=np.int64); s_off[1:] = np.cumsum(rs)
   v_off = np.zeros(nsect + 1, dtype=np.int64); v_off[1:] = np.cumsum(rs * ns)
-  up = lambda x: torch.from_numpy(np.ascontiguousarray(x, dtype=np.int64)).to(be.device)
+  up = lambda x: _up(be, x)
   st = be._stream()  # pylint: disable=protected-access
-  a_buf = be._new((int(a_off[-1]),), code)  # pylint: disable=protected-access
-  gmap = up(np.concatenate(maps) if maps else np.zeros(0, dtype=np.int64))
-  L.check(be.lib.tnb200_gather(tensor.data.t.data_ptr(), gmap.data_ptr(), a_buf.t.data_ptr(), int(a_off[-1]), code, 0, st))
   u_buf = be._new((int(u_off[-1]),), code)  # pylint: disable=protected-access
   s_buf = be._new((int(s_off[-1]),), T.real_code(code))  # pylint: disable=protected-access
   v_buf = be._new((int(v_off[-1]),), code)  # pylint: disable=protected-access
-  d_dims, d_ao, d_uo, d_so, d_vo = up(dims.reshape(-1)), up(a_off), up(u_off), up(s_off), up(v_off)
+  d_dims, d_ao, d_uo, d_so, d_vo = up(np.stack([ms, ns], axis=1).reshape(-1)), up(a_off), up(u_off), up(s_off), up(v_off)
   status = torch.zeros(1, dtype=torch.int32, device=be.device)
   rc = be.lib.tnb200_svd_batched(a_buf.t.data_ptr(), code, nsect, d_dims.data_ptr(), d_ao.data_ptr(), u_buf.t.data_ptr(),
                                  d_uo.data_ptr(), s_buf.t.data_ptr(), d_so.data_ptr(), v_buf.t.data_ptr(), d_vo.data_ptr(),
@@ -542,37 +598,71 @@ def svd(tensor, pivot_axis, max_singular_values=None, max_truncation_error=None,
     raise RuntimeError("block-sparse svd: a sector failed to converge")
   singvals = [s_host[s_off[q]:s_off[q + 1]] for q in range(nsect)]
   kept, discarded = _truncate_sectors(singvals, max_singular_values, max_truncation_error, relative)
-  # gather maps from the packed factor buffers into the block-sparse data layouts of U, S, V
-  u_idx, s_idx, v_idx, bond_q = [], [], [], []
-  for q in range(nsect):
-    k, m_, n_, r_ = kept[q], int(ms[q]), int(ns[q]), int(rs[q])
-    if k == 0:
-      continue
-    b = np.arange(k)
-    u_idx.append((u_off[q] + np.arange(m_)[None, :] * r_ + b[:, None]).ravel())      # (k x m): u_q[:, :k].T
-    v_idx.append((v_off[q] + b[:, None] * n_ + np.arange(n_)[None, :]).ravel())      # (k x n): vh_q[:k, :]
-    s_idx.append(s_off[q] + b)
-    bond_q.append(np.full(k, qn[q], dtype=np.int64))
+  U, V = _factor_tensors(tensor, nl, qn, ms, ns, kept, u_buf, u_off, v_buf, v_off)
+  s_vals = _take(be, s_buf, _cat([s_off[q] + np.arange(k) for q, k in enumerate(kept) if k]), T.real_code(code))
   ktot = int(np.sum(kept)) if kept else 0
-  cat = lambda xs: np.concatenate(xs) if xs else np.zeros(0, dtype=np.int64)
-
-  def take(buf, idx, out_code):
-    out = be._new((len(idx),), out_code)  # pylint: disable=protected-access
-    if len(idx):
-      L.check(be.lib.tnb200_gather(buf.t.data_ptr(), up(idx).data_ptr(), out.t.data_ptr(), len(idx), out_code, 0, st))
-    return out
-  u_data = take(u_buf, cat(u_idx), code)
-  v_data = take(v_buf, cat(v_idx), code)
-  s_vals = take(s_buf, cat(s_idx), T.real_code(code))
-  mod = tensor.indices[0].modulus if tensor.indices else None
-  bond_charges = cat(bond_q)
-  left = [tensor.indices[tensor.order[i]] for i in range(nl)]
-  right = [tensor.indices[tensor.order[i]] for i in range(nl, tensor.ndim)]
-  bond_u = Index(bond_charges, True, mod)
-  bond_v = Index(bond_charges, False, mod)
-  U = BlockSparseTensor(u_data, [bond_u] + left, list(range(1, nl + 1)) + [0], be)
-  V = BlockSparseTensor(v_data, [bond_v] + right, None, be)
-  assert u_data.size == BlockSparseTensor._nnz([bond_u] + left) and v_data.size == BlockSparseTensor._nnz([bond_v] + right)  # pylint: disable=protected-access
   s_disc = np.concatenate(discarded) if discarded else np.zeros(0)
-  disc_q = cat([np.full(len(d), qn[q], dtype=np.int64) for q, d in enumerate(discarded)]) if discarded else np.zeros(0, dtype=np.int64)
-  return U, dict(values=s_vals, index=bond_u, kept=kept, ktot=ktot, discarded=s_disc, discarded_charges=disc_q), V, s_disc
+  disc_q = _cat([np.full(len(d), qn[q], dtype=np.int64) for q, d in enumerate(discarded)]) if discarded else np.zeros(0, dtype=np.int64)
+  return U, dict(values=s_vals, index=U.indices[0], kept=kept, ktot=ktot, discarded=s_disc, discarded_charges=disc_q), V, s_disc
+
+
+# ===================================================================================== qr / rq
+def _wide_bytes(code):
+  """bytes of the f64 / c128 element tnb200_qr_batched computes in"""
+  return 16 if T.is_complex_code(code) else 8
+
+
+def _qr_sectors(tensor, pivot_axis, adjoint):
+  """A_q = L_q R_q for every charge sector of the matrix view (legs order[:nl] | order[nl:]): the QR of A_q (adjoint = 0:
+  L = Q, R = R) or the RQ composed from the QR of A_q^H (adjoint = 1: L = R, R = Q).  Sectors with
+  8 or 16 bytes * m n <= `_lib.QR_BATCHED_MAX_BYTES` run in ONE `tnb200_qr_batched` launch, each larger one through
+  `tnb200_qr` on its slice of the packed buffer.  No host synchronisation: the factor sizes follow from the charges."""
+  be = tensor.backend
+  nl = pivot_axis if pivot_axis >= 0 else tensor.ndim + pivot_axis
+  code = tensor.data.code
+  if code not in (L.F64, L.F32, L.C64, L.C128):
+    raise TypeError("block-sparse qr needs a float32/float64/complex tensor")
+  qn, ms, ns, a_off, a_buf = _pack_sectors(tensor, nl)
+  rs = np.minimum(ms, ns)
+  l_off = np.zeros(len(qn) + 1, dtype=np.int64); l_off[1:] = np.cumsum(ms * rs)
+  r_off = np.zeros(len(qn) + 1, dtype=np.int64); r_off[1:] = np.cumsum(rs * ns)
+  l_buf = be._new((int(l_off[-1]),), code)  # pylint: disable=protected-access
+  r_buf = be._new((int(r_off[-1]),), code)  # pylint: disable=protected-access
+  st = be._stream()  # pylint: disable=protected-access
+  elems = ms * ns
+  small = (elems > 0) & (elems * _wide_bytes(code) <= L.QR_BATCHED_MAX_BYTES)
+  batch = np.nonzero(small)[0]
+  # the kernel writes Q at q_off and R at r_off; with adjoint, R_q = R'^H is the left factor and Q_q = Q'^H the right one
+  q_buf, q_off, rr_buf, rr_off = (l_buf, l_off, r_buf, r_off) if not adjoint else (r_buf, r_off, l_buf, l_off)
+  if batch.size:
+    d_dims, d_ao = _up(be, np.stack([ms[batch], ns[batch]], axis=1).reshape(-1)), _up(be, a_off[batch])
+    d_qo, d_ro = _up(be, q_off[batch]), _up(be, rr_off[batch])
+    L.check(be.lib.tnb200_qr_batched(a_buf.t.data_ptr(), code, int(batch.size), d_dims.data_ptr(), d_ao.data_ptr(),
+                                      q_buf.t.data_ptr(), d_qo.data_ptr(), rr_buf.t.data_ptr(), d_ro.data_ptr(),
+                                      int(elems[batch].max()), int(adjoint), st))
+  for q in np.nonzero(~small & (elems > 0))[0]:
+    m_, n_, r_ = int(ms[q]), int(ns[q]), int(rs[q])
+    a_q = B200Tensor(a_buf.t[a_off[q]:a_off[q + 1]].view(m_, n_), code)
+    l_q = B200Tensor(l_buf.t[l_off[q]:l_off[q + 1]].view(m_, r_), code)
+    r_q = B200Tensor(r_buf.t[r_off[q]:r_off[q + 1]].view(r_, n_), code)
+    if not adjoint:
+      L.check(be.lib.tnb200_qr(a_q.ref(), l_q.ref(), r_q.ref(), 0, st))
+    else:
+      rr, qq = be.rq(a_q, 1)
+      L.check(be.lib.tnb200_copy(rr.ref(), l_q.ref(), 0, st))
+      L.check(be.lib.tnb200_copy(qq.ref(), r_q.ref(), 0, st))
+  return _factor_tensors(tensor, nl, qn, ms, ns, [int(r) for r in rs], l_buf, l_off, r_buf, r_off)
+
+
+def qr(tensor, pivot_axis):
+  """Block-sparse QR (block_sparse/linalg.py:300-393 behind backends/symmetric/decompositions.py:219-231): np.linalg.qr's
+  reduced factors of every charge sector.  Returns (Q, R): Q legs = left legs + [bond] (bond flow True), R legs =
+  [bond] + right legs (bond flow False); the bond carries each sector's charge min(m_q, n_q) times, ascending."""
+  return _qr_sectors(tensor, pivot_axis, 0)
+
+
+def rq(tensor, pivot_axis):
+  """Block-sparse RQ (backends/symmetric/decompositions.py:234-248): per sector, the QR of A_q^H conjugate-transposed
+  back, A_q = R_q Q_q with R_q = R'^H (m x r) and Q_q = Q'^H (r x n).  Returns (R, Q) with the leg layout of `qr`:
+  R legs = left legs + [bond] (flow True), Q legs = [bond] + right legs (flow False)."""
+  return _qr_sectors(tensor, pivot_axis, 1)

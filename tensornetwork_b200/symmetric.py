@@ -1,16 +1,19 @@
-"""`symmetric_b200`: the reference's `SymmetricBackend` with its two hot operations on the B200.
+"""`symmetric_b200`: the reference's `SymmetricBackend` with its hot operations on the B200.
 
 Reference: `tensornetwork/backends/symmetric/symmetric_backend.py:30` (class), `:38-40` (tensordot ->
 `block_sparse.tensordot`, blocksparsetensor.py:925-1108), `:50-59` (svd -> backends/symmetric/
-decompositions.py:27-216).  Registered under the name "symmetric_b200" in `backend_factory._BACKENDS`
-when the reference package is importable, so `tn.Node(BlockSparseTensor, backend="symmetric_b200")`,
-`tn.split_node*` and `FiniteDMRG` on block-sparse MPS run the grouped sector kernels
-(`tnb200_blocksparse_tensordot`, `tnb200_svd_batched`) of `tensornetwork_b200.blocksparse`.
+decompositions.py:27-216), `:61-81` (qr / rq -> decompositions.py:219-248 -> block_sparse/linalg.py:300-393).
+Registered under the name "symmetric_b200" in `backend_factory._BACKENDS` when the reference package is importable,
+so `tn.Node(BlockSparseTensor, backend="symmetric_b200")`, `tn.split_node*`, `FiniteMPS` canonicalisation and
+`FiniteDMRG` on block-sparse MPS run the grouped sector kernels (`tnb200_blocksparse_tensordot`, `tnb200_svd_batched`,
+`tnb200_qr_batched`) of `tensornetwork_b200.blocksparse`.
 
 Scope (stated, not hidden): tensors stay the reference's own `BlockSparseTensor` objects — charges, flows,
 leg fusion (`reshape`), lazy transposition and every elementwise helper on the nnz vector are the reference's
-host code, inherited unchanged; `tensordot` and `svd` — where the reference spends its time (SURVEY 8a rows
-a11, a12) — upload the nnz vectors, run on the device and download the result.  Supported symmetry: ONE
+host code, inherited unchanged; `tensordot`, `svd`, `qr` and `rq` — where the reference spends its time (SURVEY 8a
+rows a11, a12; `qr` / `rq` at every site of MPS canonicalisation and one-site DMRG) — upload the nnz vectors, run on
+the device and download the result.  `qr` / `rq` build their own sector maps, so they also factor the dimension-1
+boundary legs of a finite MPS, on which the reference's host path fails under numpy 2.  Supported symmetry: ONE
 U(1) / Z_N charge per leg (the reference's product charges raise NotImplementedError here, as do the two
 degenerate forms of tensordot that are not sector contractions: outer product and full inner product go to
 the reference implementation, which is a numpy dot / outer of the data vectors).
@@ -130,6 +133,35 @@ def _make_class():
       sdisc = ChargeArray(S["discarded"], [mk(S["discarded_charges"])], [False])
       k = s.shape[0]
       return u.reshape(tuple(left_dims) + (k,)), s, v.reshape((k,) + tuple(right_dims)), sdisc
+
+    # ------------------------------------------------------------------ qr / rq
+    def _split(self, tensor, pivot_axis, factor):
+      """(left, right) block-sparse factors of `bsp.qr` / `bsp.rq` as the reference's decompositions.qr / rq shape them:
+      left = left legs + [bond] (bond flow True), right = [bond] + right legs (bond flow False)."""
+      left_dims, right_dims = tensor.shape[:pivot_axis], tensor.shape[pivot_axis:]
+      dt, groups = _to_device(tensor, self.device_backend)
+      nl = sum(len(g) for g in groups[:len(left_dims)])
+      lf, rf = factor(dt, nl)
+      bond = type(tensor._charges[0])(np.asarray(lf.indices[0].charges, dtype=np.int16))  # pylint: disable=protected-access
+      flat = dt.order
+      cf = lambda legs: ([tensor._charges[o] for o in legs], [tensor._flows[o] for o in legs])  # pylint: disable=protected-access
+      (left_c, left_f), (right_c, right_f) = cf(flat[:nl]), cf(flat[nl:])
+      left = BlockSparseTensor(lf.data.to_host(), charges=[bond] + left_c, flows=[True] + left_f,
+                               order=[[0], list(range(1, nl + 1))], check_consistency=False).transpose((1, 0))
+      right = BlockSparseTensor(rf.data.to_host(), charges=[bond] + right_c, flows=[False] + right_f,
+                                order=[[0], list(range(1, len(right_c) + 1))], check_consistency=False)
+      k = lf.indices[0].dim
+      return left.reshape(tuple(left_dims) + (k,)), right.reshape((k,) + tuple(right_dims))
+
+    def qr(self, tensor, pivot_axis=-1, non_negative_diagonal=False):
+      if non_negative_diagonal or not isinstance(tensor, BlockSparseTensor):
+        return super().qr(tensor, pivot_axis, non_negative_diagonal)   # the reference's NotImplementedError / host path
+      return self._split(tensor, pivot_axis, bsp.qr)
+
+    def rq(self, tensor, pivot_axis=-1, non_negative_diagonal=False):
+      if non_negative_diagonal or not isinstance(tensor, BlockSparseTensor):
+        return super().rq(tensor, pivot_axis, non_negative_diagonal)
+      return self._split(tensor, pivot_axis, bsp.rq)
 
   _CLASS = SymmetricB200Backend
   return _CLASS
