@@ -260,8 +260,9 @@ TNB200_API int32_t tnb200_expm(const tnb200_tensor_t* a, const tnb200_tensor_t* 
 /* ---- a11: block_sparse.tensordot per-sector loop (block_sparse/blocksparsetensor.py:1094-1101).
  * For each sector q: C.data[c_map[q]] = A.data[a_map[q]].reshape(m_q,k_q) @ B.data[b_map[q]]
  * .reshape(k_q,n_q), all sectors in ONE launch.  maps are int64 element indices into the flat
- * data vectors, concatenated; *_off[q] is the start of sector q inside the concatenation
- * (nsect+1 entries).  dims holds (m_q, k_q, n_q) triples.  All arrays are device pointers. */
+ * data vectors; *_off[q] is where sector q's maps start, and they run for m_q k_q (a), k_q n_q (b)
+ * and m_q n_q (c) entries, with dims holding the (m_q, k_q, n_q) triples.  Offsets need not
+ * increase, and only the first nsect entries are read.  All arrays are device pointers. */
 TNB200_API int32_t tnb200_blocksparse_tensordot(const void* a_data, const void* b_data, void* c_data,
                                      int32_t dtype, int32_t nsect, const int64_t* dims_dev,
                                      const int64_t* a_map_dev, const int64_t* a_off_dev,

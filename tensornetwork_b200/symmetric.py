@@ -94,7 +94,8 @@ def _make_class():
       try:
         dc = bsp.tensordot(da, db, (ea, eb))
       except ValueError:
-        return super().tensordot(a, b, axes)            # mismatching charges / flows: raise exactly what the reference raises
+        super().tensordot(a, b, axes)                   # mismatching charges / flows: raise exactly what the reference raises
+        raise                                           # anything else, a device error included, is not the reference's
       free1 = [n for n in range(a.ndim) if n not in axes1]
       free2 = [n for n in range(b.ndim) if n not in axes2]
       charges, flows, order, s = [], [], [], 0

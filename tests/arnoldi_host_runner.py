@@ -2,49 +2,12 @@
 on a stand-in library whose tnb200_arnoldi_orth is a plain numpy CGS2 on host memory.  Checks restarts, conjugate
 pairs, breakdown, every `which`, the errors and the statistics against np.linalg.eig; the kernel itself is checked by
 tests/test_gpu_eigs.py."""
-import ctypes
-import os
-import sys
 import numpy as np
+import hostrun
+from hostrun import raises
+_, lib = hostrun.install()
+from tensornetwork_b200 import backend as tb_backend, arnoldi  # noqa: E402
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-from tensornetwork_b200 import _lib, backend as tb_backend, arnoldi
-import fake_lib
-
-
-class ArnoldiFakeLib(fake_lib.FakeLib):
-  """FakeLib plus tnb200_arnoldi_orth with the kernel's contract (include/tnb200.h)."""
-
-  def tnb200_arnoldi_orth(self, v, j, w, h_ptr, stream):
-    V, W = fake_lib._view(v), fake_lib._view(w).reshape(-1)
-    k = j + 1
-    cplx = np.iscomplexobj(V)
-    acc = np.complex128 if cplx else np.float64
-    eps = np.finfo(V.real.dtype).eps
-    Vk, x = V[:k].astype(acc), W.astype(acc)
-    h1 = Vk.conj() @ x
-    V[k] = x - Vk.T @ h1                      # stored in the basis dtype between the passes, as on the device
-    u = V[k].astype(acc)
-    h2 = Vk.conj() @ u
-    r = u - Vk.T @ h2
-    beta = np.linalg.norm(r)
-    if beta <= 16.0 * np.sqrt(k + 1.0) * eps * np.linalg.norm(x):
-      V[k] = 0
-      beta = 0.0
-    else:
-      V[k] = r / beta
-    h = np.ndarray((k + 1,), dtype=acc, buffer=(ctypes.c_char * ((k + 1) * np.dtype(acc).itemsize)).from_address(h_ptr))
-    h[:k] = h1 + h2
-    h[k] = beta
-    self._kernel = b"arnoldi_cgs2"
-    self._launches += 4
-    return 0
-
-
-_lib.set_lib(ArnoldiFakeLib())
-tb_backend._CONFIG["device"] = "cpu"
 be = tb_backend.CudaB200Backend()
 
 WHICH = ("LM", "SM", "LR", "SR")
@@ -124,11 +87,7 @@ M = from_spectrum(rng, np.concatenate([[1.0, 0.99], rng.uniform(-0.9, 0.9, 498)]
 _, _, info = check(M, "LR", 1, ncv=8)
 assert info["restarts"] >= 2, info
 assert info["host_reads"] >= info["matvecs"], info
-try:
-  run(M, "LR", 1, 8, 1e-12, maxiter=1)
-  raise SystemExit("expected RuntimeError")
-except RuntimeError as e:
-  assert "converged" in str(e)
+raises(RuntimeError, lambda: run(M, "LR", 1, 8, 1e-12, maxiter=1), match="converged")
 print("restarts ok", info)
 
 # a real operator with complex eigenvalues: rotation blocks in a random real basis
@@ -172,15 +131,6 @@ print("breakdown ok")
 x = be.convert_to_tensor(np.ones(30))
 mv = lambda v: v  # noqa: E731
 
-
-def raises(exc, f):
-  try:
-    f()
-  except exc:
-    return
-  raise SystemExit("expected {}".format(exc.__name__))
-
-
 raises(ValueError, lambda: be.eigs(mv, initial_state=x, which="LI"))
 raises(ValueError, lambda: be.eigs(mv, initial_state=x, which="SI"))
 raises(ValueError, lambda: be.eigs(mv, initial_state=x, numeig=5, num_krylov_vecs=6))
@@ -195,4 +145,4 @@ raises(ValueError, lambda: be.eigs(mv, initial_state=be.convert_to_tensor(np.zer
 eta, vecs = be.eigs(lambda v: v * 2.0, shape=(6, 5), dtype=np.float64, numeig=1, num_krylov_vecs=10)
 assert vecs[0].shape == (6, 5) and abs(eta.to_host()[0] - 2.0) < 1e-12
 print("errors ok")
-print("ARNOLDI HOST OK")
+hostrun.done(lib)

@@ -2,48 +2,13 @@
 on a stand-in library whose tnb200_arnoldi_orth is a plain numpy CGS2 on host memory.  Compares info, the matvec count
 and x with scipy.sparse.linalg.gmres on dense problems, and checks breakdown, x0, b = 0, atol and the errors; the
 kernel itself is checked by tests/test_gpu_eigs.py."""
-import ctypes
-import os
-import sys
 import numpy as np
 import scipy.sparse.linalg as spla
+import hostrun
+from hostrun import raises
+_, lib = hostrun.install()
+from tensornetwork_b200 import backend as tb_backend, gmres as tb_gmres  # noqa: E402
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-from tensornetwork_b200 import _lib, backend as tb_backend, gmres as tb_gmres
-import fake_lib
-
-
-class ArnoldiFakeLib(fake_lib.FakeLib):
-  """FakeLib plus tnb200_arnoldi_orth with the kernel's contract (include/tnb200.h)."""
-
-  def tnb200_arnoldi_orth(self, v, j, w, h_ptr, stream):
-    V, W = fake_lib._view(v), fake_lib._view(w).reshape(-1)
-    k = j + 1
-    acc = np.complex128 if np.iscomplexobj(V) else np.float64
-    eps = np.finfo(V.real.dtype).eps
-    Vk, x = V[:k].astype(acc), W.astype(acc)
-    h1 = Vk.conj() @ x
-    V[k] = x - Vk.T @ h1                      # stored in the basis dtype between the passes, as on the device
-    u = V[k].astype(acc)
-    h2 = Vk.conj() @ u
-    r = u - Vk.T @ h2
-    beta = np.linalg.norm(r)
-    if beta <= 16.0 * np.sqrt(k + 1.0) * eps * np.linalg.norm(x):
-      V[k] = 0
-      beta = 0.0
-    else:
-      V[k] = r / beta
-    h = np.ndarray((k + 1,), dtype=acc, buffer=(ctypes.c_char * ((k + 1) * np.dtype(acc).itemsize)).from_address(h_ptr))
-    h[:k] = h1 + h2
-    h[k] = beta
-    self._launches += 4
-    return 0
-
-
-_lib.set_lib(ArnoldiFakeLib())
-tb_backend._CONFIG["device"] = "cpu"
 be = tb_backend.CudaB200Backend()
 rng = np.random.default_rng(1)
 
@@ -169,14 +134,6 @@ print("backend method ok")
 
 
 # errors
-def raises(exc, f):
-  try:
-    f()
-  except exc:
-    return
-  raise SystemExit("expected {}".format(exc.__name__))
-
-
 x = be.convert_to_tensor(np.ones(30))
 mv = lambda v: v  # noqa: E731
 raises(ValueError, lambda: be.gmres(mv, x, x0=be.convert_to_tensor(np.ones(31))))
@@ -199,4 +156,4 @@ raises(ValueError, lambda: be.gmres(lambda v: be.reshape(v, (5, 6)), x))
 y, info = be.gmres(lambda v: v * 2.0, x, num_krylov_vectors=40)
 assert info == 0 and np.allclose(y.to_host(), 0.5)
 print("errors ok")
-print("GMRES HOST OK")
+hostrun.done(lib)

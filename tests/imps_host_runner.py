@@ -1,138 +1,16 @@
 """Runs in a subprocess (build container only): the reference's own InfiniteMPS.canonicalize on backend="cuda_b200",
-on a stand-in library that adds numpy versions of tnb200_eigh, tnb200_arnoldi_orth, tnb200_compare,
-tnb200_index_update, tnb200_lu_factor and tnb200_inv with the contracts of include/tnb200.h.  Checks the adapter's host
-logic against backend="numpy": canonicalize's results, the comparison / index_update semantics and inv's errors.  The
-kernels themselves are checked by tests/test_gpu_inv.py and tests/test_gpu_canonicalize.py."""
-import ctypes
-import os
-import sys
+on the stand-in library tests/fake_lib.FakeLib, whose tnb200_eigh, tnb200_arnoldi_orth, tnb200_compare,
+tnb200_index_update, tnb200_lu_factor and tnb200_inv are numpy versions with the contracts of include/tnb200.h.  Checks
+the adapter's host logic against backend="numpy": canonicalize's results, the comparison / index_update semantics and
+inv's errors.  The kernels themselves are checked by tests/test_gpu_inv.py and tests/test_gpu_canonicalize.py."""
 import numpy as np
-import scipy.linalg
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-from baseline import refenv  # noqa: E402
-tn = refenv.load()
-from tensornetwork_b200 import _lib, backend as tb_backend  # noqa: E402
-from tensornetwork_b200.tensor import B200Tensor  # noqa: E402
-import fake_lib  # noqa: E402
-
-
-def _view(arg):
-  """fake_lib._view plus the one-byte bool mask dtype"""
-  d = fake_lib._desc(arg)
-  if d.dtype != _lib.BOOL:
-    return fake_lib._view(arg)
-  shape = tuple(d.shape[i] for i in range(d.ndim))
-  if any(s == 0 for s in shape):
-    return np.zeros(shape, dtype=bool)
-  span = sum((s - 1) * abs(d.stride[i]) for i, s in enumerate(shape)) + 1
-  buf = (ctypes.c_char * span).from_address(d.data)
-  return np.ndarray(shape, dtype=bool, buffer=buf, strides=tuple(d.stride[i] for i in range(d.ndim)))
-
-
-def _ivec(ptr, n):
-  return np.ndarray((n,), dtype=np.int32, buffer=(ctypes.c_char * (4 * max(n, 1))).from_address(int(ptr)))
-
-
-class ImpsFakeLib(fake_lib.FakeLib):
-  """FakeLib plus the entry points InfiniteMPS.canonicalize reaches, with the contracts of include/tnb200.h."""
-
-  def tnb200_eigh(self, a, w, v, info, stream):
-    ww, vv = np.linalg.eigh(_view(a))
-    _view(w)[...] = ww
-    _view(v)[...] = vv
-    return 0
-
-  def tnb200_arnoldi_orth(self, v, j, w, h_ptr, stream):
-    V, W = _view(v), _view(w).reshape(-1)
-    k = j + 1
-    acc = np.complex128 if np.iscomplexobj(V) else np.float64
-    eps = np.finfo(V.real.dtype).eps
-    Vk, x = V[:k].astype(acc), W.astype(acc)
-    h1 = Vk.conj() @ x
-    V[k] = x - Vk.T @ h1
-    u = V[k].astype(acc)
-    h2 = Vk.conj() @ u
-    r = u - Vk.T @ h2
-    beta = np.linalg.norm(r)
-    if beta <= 16.0 * np.sqrt(k + 1.0) * eps * np.linalg.norm(x):
-      V[k] = 0
-      beta = 0.0
-    else:
-      V[k] = r / beta
-    h = np.ndarray((k + 1,), dtype=acc, buffer=(ctypes.c_char * ((k + 1) * np.dtype(acc).itemsize)).from_address(h_ptr))
-    h[:k] = h1 + h2
-    h[k] = beta
-    return 0
-
-  def tnb200_compare(self, op, a, b, c, stream):
-    A, B = _view(a), _view(b)
-    if fake_lib._desc(c).dtype != _lib.BOOL:
-      return self._fail(-1, "compare: the output must be a bool mask")
-    if np.iscomplexobj(A) or np.iscomplexobj(B):
-      return self._fail(-2, "compare: complex values are not ordered")
-    _view(c)[...] = (np.less, np.less_equal, np.greater, np.greater_equal)[op](A, B)
-    self._launches += 1
-    return 0
-
-  def tnb200_index_update(self, a, mask, re, im, value_ptr, value_dtype, out, stream):
-    A, O = _view(a), _view(out)
-    if value_ptr:
-      value = fake_lib._scalar_at(value_ptr, value_dtype)[()]
-    else:
-      value = complex(re, im) if im != 0.0 else re
-    if np.iscomplexobj(value) and not np.iscomplexobj(A):
-      return self._fail(-2, "index_update: cannot assign a complex value to a real tensor")
-    if A.dtype.kind == "i" and np.asarray(value).dtype.kind in "fc":
-      value = np.trunc(np.real(value))
-    M = np.ones(A.shape, bool) if not mask else _view(mask)
-    O[...] = np.where(M, np.asarray(value).astype(A.dtype), A)
-    self._launches += 1
-    return 0
-
-  @staticmethod
-  def _factor(A):
-    lu, piv = scipy.linalg.lu_factor(A.astype(np.complex128 if np.iscomplexobj(A) else np.float64), check_finite=False)
-    zero = np.flatnonzero(np.diagonal(lu) == 0)
-    return lu, piv, (int(zero[0]) + 1 if zero.size else 0)
-
-  def tnb200_lu_factor(self, a, lu, piv_ptr, info_ptr, stream):
-    A = _view(a)
-    if A.shape[0] != A.shape[1]:
-      return self._fail(-1, "lu_factor: the matrix must be square")
-    f, p, info = self._factor(A)
-    _view(lu)[...] = f
-    _ivec(piv_ptr, A.shape[0])[...] = p
-    _ivec(info_ptr, 1)[0] = info
-    return 0
-
-  def tnb200_inv(self, a, x, info_ptr, stream):
-    A = _view(a)
-    if A.shape[0] != A.shape[1]:
-      return self._fail(-1, "inv: the matrix must be square")
-    _, _, info = self._factor(A)
-    _ivec(info_ptr, 1)[0] = info
-    if info == 0:
-      _view(x)[...] = np.linalg.inv(A)
-    self._launches += 1
-    return 0
-
-
-_lib.set_lib(ImpsFakeLib())
-tb_backend._CONFIG["device"] = "cpu"
-import tensornetwork_b200  # noqa: E402,F401  pylint: disable=unused-import  (registers "cuda_b200")
+import hostrun
+from hostrun import raises
+tn, lib = hostrun.install(reference=True)
 from tensornetwork.matrixproductstates.infinite_mps import InfiniteMPS  # noqa: E402
+from tensornetwork_b200 import backend as tb_backend  # noqa: E402
+from tensornetwork_b200.tensor import B200Tensor  # noqa: E402
 be = tb_backend.get_instance()
-
-
-def raises(exc, f):
-  try:
-    f()
-  except exc:
-    return
-  raise SystemExit("expected {}".format(exc.__name__))
 
 
 def schmidt(connector):
@@ -258,4 +136,4 @@ m = rng.standard_normal((5, 5))
 out = tn_linalg.inv(tn.Tensor(be.convert_to_tensor(m), backend="cuda_b200"))
 np.testing.assert_allclose(np.asarray(out.array), np.linalg.inv(m), rtol=1e-10)
 print("inv ok")
-print("IMPS HOST OK")
+hostrun.done(lib)

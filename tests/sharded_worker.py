@@ -10,18 +10,11 @@ The device layer is tests/fake_lib.FakeLib (host memory), torch.distributed runs
   * (SHARDED_EXPECT_REFUSAL=1) a plan the model rejects is refused on every rank before anything is posted.
 """
 import os
-import sys
 import numpy as np
 import torch.distributed as dist
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-from tensornetwork_b200 import _lib, backend as tb_backend  # noqa: E402
-import fake_lib  # noqa: E402
-_lib.set_lib(fake_lib.FakeLib())
-tb_backend._CONFIG["device"] = "cpu"
-from tensornetwork_b200 import drivers, parallel  # noqa: E402
+import hostrun
+hostrun.install()
+from tensornetwork_b200 import backend as tb_backend, drivers, parallel  # noqa: E402
 from oracle import np_network as nn  # noqa: E402
 import bench  # noqa: E402
 

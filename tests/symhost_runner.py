@@ -1,27 +1,16 @@
 """Runs in a subprocess: the symmetric_b200 adapter (tensornetwork_b200/symmetric.py) driven by the REAL reference's callers
-(block-sparse tn.Node @, split_node, ncon, backend.svd) with the device layer replaced by tests/fake_lib.FakeLib (host memory):
-checks the conversion between the reference's BlockSparseTensor and the elementary-leg form the kernels take."""
-import os, sys
+(the tests of tests/test_gpu_symmetric_adapter.py: block-sparse tn.Node @, split_node, ncon, backend.svd) with the device
+layer replaced by tests/fake_lib.FakeLib (host memory): checks the conversion between the reference's BlockSparseTensor
+and the elementary-leg form the kernels take, and that errors surface as the reference raises them."""
 import numpy as np
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
-from baseline import refenv
-tn = refenv.load()
-from tensornetwork_b200 import _lib, backend as tb_backend
-import fake_lib
-_lib.set_lib(fake_lib.FakeLib())
-tb_backend._CONFIG["device"] = "cpu"
-import tensornetwork_b200 as tb
+import hostrun
+tn, lib = hostrun.install(reference=True)
+import tensornetwork_b200 as tb  # noqa: E402
+from tensornetwork_b200 import _lib  # noqa: E402
 assert tb.registered_symmetric
-import importlib.util, types
-spec = importlib.util.spec_from_file_location("tsym", os.path.join(ROOT, "tests", "test_gpu_symmetric_adapter.py"))
-m = importlib.util.module_from_spec(spec); spec.loader.exec_module(m)
-m.test_registered_and_tensordot_matches_reference(tn); print("tensordot ok")
-m.test_nodes_and_split_node_on_blocksparse_tensors(tn); print("nodes/split ok")
-for kw in [{}, {"max_singular_values": 7}, {"max_truncation_error": 0.2}, {"max_truncation_error": 0.1, "relative": True}]:
-    m.test_svd_matches_reference(tn, kw)
-print("svd ok")
-m.test_ncon_two_site_matvec_on_blocksparse_tensors(tn); print("ncon ok")
+hostrun.run_gpu_tests("test_gpu_symmetric_adapter.py", tn, lib)
+# the contractions ran through the stand-in's kernel contract, not around it
+assert lib.calls["tnb200_blocksparse_tensordot"] and not lib.raised["tnb200_blocksparse_tensordot"], (lib.calls, lib.raised)
 
 # ---- device-side map construction (csrc/blocksparse_maps.cu; FakeLib carries a numpy transcription of the same five
 # stages): the host tables (charge-degeneracy arithmetic) + the algorithm reproduce the lexsort-built maps exactly
@@ -54,4 +43,14 @@ gu, gs, gv, _ = _be.svd(za, 2)
 wu, ws, wv, _ = _ref.svd(za, 2)
 assert np.allclose(gs.data, ws.data, atol=1e-10), "Z3 svd"
 print("Z_N ok")
-print("SYMHOST OK")
+
+# errors: a device error surfaces instead of becoming the reference's host result; mismatched legs raise the reference's
+# own message
+lib.tnb200_blocksparse_tensordot = lambda *args: lib._fail(_lib.ERR_INVALID, "blocksparse: rejected by the stand-in")
+hostrun.raises(ValueError, _be.tensordot, za, zb, ([2, 3], [1, 0]), match="rejected by the stand-in")
+del lib.tnb200_blocksparse_tensordot
+zs = tn.BlockSparseTensor.random([zl[3].copy(), zl[2].copy().flip_flow(), zl[0].copy()], dtype=np.float64)
+assert (str(hostrun.raises(ValueError, _be.tensordot, za, zs, ([2, 3], [1, 0])))
+        == str(hostrun.raises(ValueError, _ref.tensordot, za, zs, ([2, 3], [1, 0]))))
+print("errors ok")
+hostrun.done(lib)
