@@ -309,7 +309,8 @@ TNB200_API int32_t tnb200_qr_batched(const void* a_data, int32_t dtype, int32_t 
  * into the two groups whose states are enumerated; shift = sum of max|charge| over the legs (U(1)), modulus = N for Z_N
  * (0: U(1)); nbins = 2*shift+1 or N; tables_dev = int64 [start_right(nbins) | sect_off(nbins) | ncols(nbins)], the
  * per-charge tables the caller derives from the legs' charge histograms (charge-degeneracy arithmetic).
- * dims / leg_off / order are HOST arrays. */
+ * dims / leg_off / order are HOST arrays.  This is tnb200_blocksparse_maps_nsym (include/tnb200_symmetry.h) with
+ * nsym = 1. */
 TNB200_API int32_t tnb200_blocksparse_maps(int32_t nlegs, const int64_t* dims, const int64_t* charges_dev, const int64_t* leg_off,
                                            const int32_t* order, int32_t partition, int32_t split, int64_t modulus, int64_t shift,
                                            int32_t nbins, const int64_t* tables_dev, int64_t nnz, int64_t* map_dev, void* stream);

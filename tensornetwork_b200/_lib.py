@@ -25,6 +25,10 @@ MATH_DEFAULT, MATH_STRICT, MATH_SIMT = 0 << 4, 1 << 4, 2 << 4
 EXPM_FUSED_MAX_N = 48
 # TNB200_QR_BATCHED_MAX_BYTES: tnb200_qr_batched takes problems with sizeof(f64 or c128) * m * n up to this
 QR_BATCHED_MAX_BYTES = 200 * 1024
+# TNB200_BLOCKSPARSE_MAX_NSYM / _MAX_BINS (include/tnb200_symmetry.h): charge components per leg and charge bins
+# tnb200_blocksparse_maps_nsym takes
+BLOCKSPARSE_MAX_NSYM = 8
+BLOCKSPARSE_MAX_BINS = 1 << 22
 
 
 class TensorDesc(ctypes.Structure):
@@ -93,6 +97,11 @@ SIGNATURES = {
     "tnb200_thin_run_destroy": (_i32, [_vp]),
 }
 
+# name -> (restype, argtypes): every symbol include/tnb200_symmetry.h declares (product charges on block-sparse legs)
+SYMMETRY_SIGNATURES = {
+    "tnb200_blocksparse_maps_nsym": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _i64, _vp, _vp]),
+}
+
 _lib = None
 
 
@@ -106,7 +115,7 @@ def load(path=None):
     raise OSError("libtnb200.so not found at {} — build it with "
                   "`python -m tensornetwork_b200.build` (there is no CPU fallback)".format(path))
   lib = ctypes.CDLL(path)
-  for name, (res, args) in SIGNATURES.items():
+  for name, (res, args) in list(SIGNATURES.items()) + list(SYMMETRY_SIGNATURES.items()):
     fn = getattr(lib, name)
     fn.restype = res
     fn.argtypes = args

@@ -1,4 +1,4 @@
-"""Abelian-symmetric (U(1) / Z_N) block-sparse tensors on the `cuda_b200` backend.
+"""Abelian-symmetric (U(1) / Z_N, and products of them) block-sparse tensors on the `cuda_b200` backend.
 
 Covers SURVEY.md 8(a) row a11: `block_sparse.tensordot`
 (tensornetwork/block_sparse/blocksparsetensor.py:925-1108) with its index maps
@@ -16,6 +16,8 @@ per (charges, flows, order, partition) signature on the host (pure integer work,
 checked bit-exactly against the reference's maps in tests/) and ALL sectors run in ONE launch
 of the grouped kernel `tnb200_blocksparse_tensordot`.
 """
+import math
+
 import numpy as np
 from . import _lib as L
 from . import tensor as T
@@ -25,31 +27,130 @@ _MAP_CACHE = {}
 
 
 class Index:
-  """One tensor leg: an integer charge per basis state and a flow (True = outflowing), the
-  information content of `block_sparse.Index` (index.py) for a single Abelian symmetry."""
+  """One tensor leg: a charge per basis state and a flow (True = outflowing), the information content of
+  `block_sparse.Index` (index.py).  One Abelian symmetry: charges of shape (dim,), modulus None (U(1)) or N (Z_N).  A
+  product of nsym symmetries (the reference's BaseCharge with nsym charge_types): charges of shape (dim, nsym) and
+  modulus a tuple with one such entry per component (a single value applies to every component).  A (dim, 1) array or a
+  1-tuple is the single-symmetry leg."""
 
   def __init__(self, charges, flow, modulus=None):
-    self.charges = np.asarray(charges, dtype=np.int64).ravel()
+    charges = np.asarray(charges, dtype=np.int64)
+    mods = tuple(modulus) if isinstance(modulus, (tuple, list)) else None
     self.flow = bool(flow)
-    self.modulus = modulus  # None: U(1); N: Z_N
+    if charges.ndim == 2 and charges.shape[1] > 1:
+      nsym = charges.shape[1]
+      mods = mods if mods is not None else (modulus,) * nsym
+      if len(mods) != nsym:
+        raise ValueError("{} moduli for {} charge components".format(len(mods), nsym))
+      self.charges = charges
+      self.modulus = tuple(None if m is None else int(m) for m in mods)
+    else:
+      if mods is not None and len(mods) != 1:
+        raise ValueError("{} moduli for 1 charge component".format(len(mods)))
+      self.charges = charges.ravel()
+      self.modulus = mods[0] if mods is not None else modulus  # None: U(1); N: Z_N
 
   @property
   def dim(self):
     return int(self.charges.shape[0])
 
+  @property
+  def nsym(self):
+    return 1 if self.charges.ndim == 1 else int(self.charges.shape[1])
+
   def flip_flow(self):
     return Index(self.charges, not self.flow, self.modulus)
 
   def key(self):
-    return (self.charges.tobytes(), self.flow, self.modulus)
+    if self.nsym == 1:
+      return (self.charges.tobytes(), self.flow, self.modulus)
+    return (self.charges.tobytes(), self.nsym, self.flow, self.modulus)
 
 
 def _signed(ix):
   return -ix.charges if ix.flow else ix.charges
 
 
+def _q2(ix):
+  """signed charges as (dim, nsym)"""
+  q = _signed(ix)
+  return q.reshape(q.shape[0], ix.nsym)
+
+
+def _mods(ix):
+  return ix.modulus if ix.nsym > 1 else (ix.modulus,)
+
+
+def _sym(indices):
+  """(nsym, per-component moduli) of a tensor's legs, from its first leg; legs with another number of components, or a
+  product leg with other moduli, raise ValueError"""
+  if not indices:
+    return 1, (None,)
+  nsym, mods = indices[0].nsym, _mods(indices[0])
+  for ix in indices[1:]:
+    if ix.nsym != nsym or (nsym > 1 and _mods(ix) != mods):
+      raise ValueError("legs with different symmetries: {} and {} components, moduli {} and {}".format(
+          nsym, ix.nsym, mods, _mods(ix)))
+  return nsym, mods
+
+
+def _wrap(q, mods):
+  """(n, nsym) charges with every Z_N column reduced mod N"""
+  q = np.array(q, dtype=np.int64, copy=True)
+  for k, m in enumerate(mods):
+    if m:
+      q[:, k] = np.mod(q[:, k], m)
+  return q
+
+
+def _shifts(indices, mods):
+  """per component: sum over the legs of max |charge| (U(1)), 0 (Z_N)"""
+  qs = [_q2(ix) for ix in indices]
+  return tuple(0 if m else int(sum(int(np.abs(q[:, k]).max()) if q.size else 0 for q in qs)) for k, m in enumerate(mods))
+
+
+def _unique_charges(q):
+  """Distinct charges in the reference's sector order, and the label of every input charge (an index into them).
+
+  q is (n,) for one symmetry or (n, nsym).  The reference orders sectors, and with them the bond charges of svd / qr / rq,
+  by block_sparse.utils.unique / intersect, whose `collapse` views each int16 charge row as one wider integer before
+  np.unique: one component sorts ascending; two sort by component 1 signed, then component 0 read as unsigned 16-bit;
+  three get a zero fourth column and sort as an int64 (every component unsigned); four sort as an int64 (component 3
+  signed, the rest unsigned); five or more are not collapsed and sort row-lexicographically (np.unique(axis=0)).
+  Product charges must fit in int16, the reference's storage type (ValueError otherwise)."""
+  q = np.asarray(q)
+  if q.ndim == 1:
+    return np.unique(q, return_inverse=True)
+  n, w = q.shape
+  if w == 1:
+    u, inv = np.unique(q[:, 0], return_inverse=True)
+    return u[:, None], inv.ravel()
+  if q.size and (q.min() < np.iinfo(np.int16).min or q.max() > np.iinfo(np.int16).max):
+    raise ValueError("product charges must fit in int16, got values in [{}, {}]".format(int(q.min()), int(q.max())))
+  a = np.ascontiguousarray(q, dtype=np.int16)
+  if w > 4:
+    u, inv = np.unique(a, axis=0, return_inverse=True)
+    return u.astype(np.int64), inv.ravel()
+  if w == 3:
+    a = np.concatenate([a, np.zeros((n, 1), dtype=np.int16)], axis=1)
+  key = a.view(np.int32 if w == 2 else np.int64).ravel()
+  _, first, inv = np.unique(key, return_index=True, return_inverse=True)
+  return q[first].astype(np.int64), inv.ravel()
+
+
+def _qkey(q):
+  """a sector charge as a dict key: an int (one symmetry) or a tuple"""
+  return int(q) if np.ndim(q) == 0 else tuple(int(x) for x in q)
+
+
 def _fused_dense(indices, mod):
-  """fused (signed) charge of every state of the product space of `indices`, row-major"""
+  """fused (signed) charge of every state of the product space of `indices`, row-major; `mod` a tuple of per-component
+  moduli gives (states, nsym)"""
+  if isinstance(mod, tuple):
+    fused = np.zeros((1, len(mod)), dtype=np.int64)
+    for ix in indices:
+      fused = (fused[:, None, :] + _q2(ix)[None, :, :]).reshape(-1, len(mod))
+    return _wrap(fused, mod)
   fused = np.zeros(1, dtype=np.int64)
   for ix in indices:
     fused = np.add.outer(fused, _signed(ix)).ravel()
@@ -65,6 +166,7 @@ def _fused_allowed(indices):
   of charge -q_l: position = l * |right| + r.  O(|left| + |right| + nnz)."""
   if not indices:
     return np.zeros(1, dtype=np.int64)
+  nsym, mods = _sym(indices)
   mod = indices[0].modulus
   dims = [ix.dim for ix in indices]
   total = 1
@@ -79,9 +181,14 @@ def _fused_allowed(indices):
   ql = _fused_dense(indices[:k], mod)
   qr = _fused_dense(indices[k:], mod)
   nr = qr.shape[0]
+  if nsym > 1:                               # label the charge rows, then match labels
+    want = _wrap(-ql, mods)
+    _, lab = np.unique(np.concatenate([qr, want]), axis=0, return_inverse=True)
+    qr, want = lab.ravel()[:nr], lab.ravel()[nr:]
+  else:
+    want = np.mod(-ql, mod) if mod else -ql
   order = np.argsort(qr, kind="stable")
   uniq, start, cnt = np.unique(qr[order], return_index=True, return_counts=True)
-  want = np.mod(-ql, mod) if mod else -ql
   idx = np.searchsorted(uniq, want)
   idx_c = np.minimum(idx, uniq.shape[0] - 1)
   valid = (idx < uniq.shape[0]) & (uniq[idx_c] == want)
@@ -99,8 +206,9 @@ def _sector_maps(indices, order, partition):
   """Gather maps of the matrix view (legs order[:partition] | legs order[partition:]).
 
   Returns (qnums, dims (nsect x 2), maps list) where maps[q] lists, row-major over the sector's
-  (rows x cols), the positions inside the flat data vector.  Sectors are ordered by ascending
-  row charge (the reference's `intersect`/`unique` ordering, blocksparse_utils.py:375-380)."""
+  (rows x cols), the positions inside the flat data vector.  qnums are the signed row charges, (nsect,) for one
+  symmetry, (nsect, nsym) for a product; sectors are in the reference's `intersect` / `unique` order
+  (blocksparse_utils.py:375-380, `_unique_charges`), ascending for one symmetry."""
   key = ("sect", tuple(ix.key() for ix in indices), tuple(order), partition)
   hit = _MAP_CACHE.get(key)
   if hit is not None:
@@ -108,22 +216,22 @@ def _sector_maps(indices, order, partition):
   pos = _fused_allowed(indices)                       # sorted => data index = rank
   dims = [ix.dim for ix in indices]
   multi = np.unravel_index(pos, dims) if dims else ()
-  mod = indices[0].modulus if indices else None
+  nsym, mods = _sym(indices)
   rows = [order[i] for i in range(partition)]
   cols = [order[i] for i in range(partition, len(order))]
   R = np.zeros(pos.shape[0], dtype=np.int64)
-  rq = np.zeros(pos.shape[0], dtype=np.int64)
+  rq = np.zeros((pos.shape[0], nsym), dtype=np.int64)
   for leg in rows:
     R = R * dims[leg] + multi[leg]
-    rq = rq + _signed(indices[leg])[multi[leg]]
+    rq = rq + _q2(indices[leg])[multi[leg]]
   C = np.zeros(pos.shape[0], dtype=np.int64)
   for leg in cols:
     C = C * dims[leg] + multi[leg]
-  if mod:
-    rq = np.mod(rq, mod)
-  perm = np.lexsort((C, R, rq))
-  rq_s = rq[perm]
-  qnums, starts, counts = np.unique(rq_s, return_index=True, return_counts=True)
+  rq = _wrap(rq, mods)
+  qnums, lab = _unique_charges(rq if nsym > 1 else rq[:, 0])
+  perm = np.lexsort((C, R, lab))
+  counts = np.bincount(lab, minlength=qnums.shape[0])
+  starts = np.cumsum(counts) - counts
   maps, sdims = [], []
   for s, c in zip(starts, counts):
     idx = perm[s:s + c]
@@ -138,7 +246,11 @@ def _sector_maps(indices, order, partition):
 def _group_hist(indices, legs, shift, mod, nbins):
   """Number of states of the product space of `legs` per fused signed charge, in the global charge bins
   (U(1): bin = q + shift; Z_N: bin = q mod N): charge-degeneracy arithmetic — a convolution of the legs' charge
-  histograms; the product space itself is never enumerated."""
+  histograms; the product space itself is never enumerated.  For product charges `shift` and `mod` are per-component
+  tuples, and the bins are mixed-radix numbers over the component bins (component 0 most significant, as
+  tnb200_blocksparse_maps_nsym numbers them): an nsym-dimensional convolution, wrapping around on Z_N axes."""
+  if isinstance(mod, tuple):
+    return _group_hist_nd(indices, legs, shift, mod)
   if mod:
     h = np.zeros(mod, dtype=np.int64)
     h[0] = 1
@@ -161,10 +273,44 @@ def _group_hist(indices, legs, shift, mod, nbins):
   return out
 
 
+def _group_hist_nd(indices, legs, shifts, mods):
+  radix = [m if m else 2 * s + 1 for m, s in zip(mods, shifts)]
+  nsym = len(mods)
+  h = np.zeros([m if m else 1 for m in mods], dtype=np.int64)
+  h[(0,) * nsym] = 1
+  lo = [0] * nsym                            # charge of index 0 on each U(1) axis
+  for t in legs:
+    q = _wrap(_q2(indices[t]), mods)
+    if q.shape[0] == 0:
+      return np.zeros(int(np.prod(radix)), dtype=np.int64)
+    qmin = np.array([0 if m else int(q[:, k].min()) for k, m in enumerate(mods)], dtype=np.int64)
+    rel = q - qmin
+    u, cnt = np.unique(rel, axis=0, return_counts=True)
+    out = np.zeros([h.shape[k] + (0 if m else int(rel[:, k].max())) for k, m in enumerate(mods)], dtype=np.int64)
+    for row, c in zip(u, cnt):
+      src = h
+      for k, m in enumerate(mods):
+        if m and row[k]:
+          src = np.roll(src, int(row[k]), axis=k)
+      out[tuple(slice(None) if m else slice(int(row[k]), int(row[k]) + h.shape[k]) for k, m in enumerate(mods))] += c * src
+    h = out
+    lo = [lo[k] + int(qmin[k]) for k in range(nsym)]
+  full = np.zeros(radix, dtype=np.int64)
+  full[tuple(slice(None) if m else slice(lo[k] + shifts[k], lo[k] + shifts[k] + h.shape[k])
+             for k, m in enumerate(mods))] = h
+  return full.ravel()
+
+
 def _count_allowed(indices):
   """number of stored elements (total signed charge zero) from the legs' charge histograms alone"""
   if not indices:
     return 1
+  nsym, mods = _sym(indices)
+  if nsym > 1:
+    shifts = _shifts(indices, mods)
+    h = _group_hist(indices, list(range(len(indices))), shifts, mods, None)
+    zero = np.ravel_multi_index([0 if m else s for m, s in zip(mods, shifts)], [m if m else 2 * s + 1 for m, s in zip(mods, shifts)])
+    return int(h[zero])
   mod = indices[0].modulus
   shift = 0 if mod else int(sum(int(np.abs(_signed(ix)).max()) if ix.dim else 0 for ix in indices))
   nbins = int(mod) if mod else 2 * shift + 1
@@ -173,10 +319,11 @@ def _count_allowed(indices):
 
 
 def _device_sector_maps(be, indices, order, partition):
-  """`_sector_maps` with the element map built ON THE DEVICE (tnb200_blocksparse_maps; SURVEY 8f rank 3).
+  """`_sector_maps` with the element map built ON THE DEVICE (tnb200_blocksparse_maps, or tnb200_blocksparse_maps_nsym for
+  product charges; SURVEY 8f rank 3).
 
-  Returns (qnums, dims (nsect x 2), dev_map (1-D int64 device tensor, all sectors, ascending charge), offs (nsect + 1)).
-  The host computes only the per-charge tables (a few dozen integers: histogram convolutions of the legs)."""
+  Returns (qnums, dims (nsect x 2), dev_map (1-D int64 device tensor, all sectors in `_sector_maps`' order), offs (nsect + 1)).
+  The host computes only the per-charge tables (histogram convolutions of the legs)."""
   key = ("dsect", tuple(ix.key() for ix in indices), tuple(order), partition)
   hit = _MAP_CACHE.get(key)
   if hit is not None:
@@ -189,12 +336,20 @@ def _device_sector_maps(be, indices, order, partition):
            np.array([0, 1], dtype=np.int64))
     _MAP_CACHE[key] = out
     return out
-  mod = indices[0].modulus if indices else None
+  nsym, mods = _sym(indices)
   dims = [ix.dim for ix in indices]
-  signed = [_signed(ix).astype(np.int64) for ix in indices]
-  shift = 0 if mod else int(sum(int(np.abs(q).max()) if q.size else 0 for q in signed))
-  nbins = int(mod) if mod else 2 * shift + 1
-  partner = (lambda b: (mod - b) % mod) if mod else (lambda b: 2 * shift - b)
+  signed = [_q2(ix) for ix in indices]
+  shifts = _shifts(indices, mods)
+  radix = [m if m else 2 * s_ + 1 for m, s_ in zip(mods, shifts)]
+  nbins = math.prod(radix)
+  if nbins > L.BLOCKSPARSE_MAX_BINS:
+    raise NotImplementedError("block-sparse maps: the charges span {} bins, more than the {} the device map builder "
+                              "takes".format(nbins, L.BLOCKSPARSE_MAX_BINS))
+  comp = [np.arange(nbins)] if nsym == 1 else np.unravel_index(np.arange(nbins), radix)   # per-component bin of every bin
+  pcomp = [(m - c) % m if m else 2 * s_ - c for c, m, s_ in zip(comp, mods, shifts)]
+  pb = pcomp[0] if nsym == 1 else np.ravel_multi_index(pcomp, radix)
+  hist = ((lambda legs: _group_hist(indices, legs, shifts[0], mods[0], nbins)) if nsym == 1 else
+          (lambda legs: _group_hist(indices, legs, shifts, mods, nbins)))
   # split of the STORED legs into two balanced groups (as _fused_allowed does)
   total, best, split, left = int(np.prod(dims)) if dims else 1, None, 1, 1
   for i in range(1, n + 1):
@@ -204,33 +359,43 @@ def _device_sector_maps(be, indices, order, partition):
       best, split = cost, i
   stored = list(range(n))
   rows, cols = list(order[:partition]), list(order[partition:])
-  h_left = _group_hist(indices, stored[:split], shift, mod, nbins)
-  h_right = _group_hist(indices, stored[split:], shift, mod, nbins)
-  h_row = _group_hist(indices, rows, shift, mod, nbins)
-  h_col = _group_hist(indices, cols, shift, mod, nbins)
-  pb = np.array([partner(b) for b in range(nbins)], dtype=np.int64)
+  h_left = hist(stored[:split])
+  h_right = hist(stored[split:])
+  h_row = hist(rows)
+  h_col = hist(cols)
   nnz = int((h_left * h_right[pb]).sum())
   start_right = np.zeros(nbins, dtype=np.int64)
   start_right[1:] = np.cumsum(h_right)[:-1]
   ncols = h_col[pb]
   sizes = h_row * ncols
-  sect_off = np.zeros(nbins, dtype=np.int64)
-  sect_off[1:] = np.cumsum(sizes)[:-1]
   live = np.nonzero(sizes > 0)[0]
-  qnums = live.astype(np.int64) if mod else (live - shift).astype(np.int64)
+  # the sectors' charges, laid out in the reference's order (ascending bins for one symmetry)
+  if nsym == 1:
+    qnums = (live - shifts[0]).astype(np.int64)
+  else:
+    qnums, lab = _unique_charges(np.stack([comp[k][live] - shifts[k] for k in range(nsym)], axis=1).astype(np.int64))
+    live = live[np.argsort(lab)]
+  sect_off = np.zeros(nbins, dtype=np.int64)
+  sect_off[live] = np.cumsum(sizes[live]) - sizes[live]
   sdims = np.stack([h_row[live], ncols[live]], axis=1).astype(np.int64).reshape(-1, 2)
   offs = np.append(sect_off[live], nnz).astype(np.int64)
   assert int(sizes.sum()) == nnz
   leg_off = np.zeros(n, dtype=np.int64)
   leg_off[1:] = np.cumsum(dims)[:-1]
-  charges_dev = torch.from_numpy(np.concatenate(signed) if signed else np.zeros(1, dtype=np.int64)).to(be.device)
+  charges_dev = torch.from_numpy(np.ascontiguousarray(np.concatenate(signed)).ravel()).to(be.device)
   tables_dev = torch.from_numpy(np.concatenate([start_right, sect_off, ncols])).to(be.device)
   dev_map = torch.empty(max(nnz, 1), dtype=torch.int64, device=be.device)
   i64 = lambda xs: (ctypes.c_int64 * max(len(xs), 1))(*[int(x) for x in xs])
   i32 = lambda xs: (ctypes.c_int32 * max(len(xs), 1))(*[int(x) for x in xs])
-  L.check(be.lib.tnb200_blocksparse_maps(n, i64(dims), charges_dev.data_ptr(), i64(leg_off), i32(order), int(partition), int(split),
-                                          int(mod or 0), int(shift), nbins, tables_dev.data_ptr(), nnz, dev_map.data_ptr(),
-                                          be._stream()))  # pylint: disable=protected-access
+  st = be._stream()  # pylint: disable=protected-access
+  if nsym == 1:
+    rc = be.lib.tnb200_blocksparse_maps(n, i64(dims), charges_dev.data_ptr(), i64(leg_off), i32(order), int(partition), int(split),
+                                        int(mods[0] or 0), int(shifts[0]), nbins, tables_dev.data_ptr(), nnz, dev_map.data_ptr(), st)
+  else:
+    rc = be.lib.tnb200_blocksparse_maps_nsym(n, nsym, i64(dims), charges_dev.data_ptr(), i64(leg_off), i32(order), int(partition),
+                                             int(split), i64([m or 0 for m in mods]), i64(shifts), nbins, tables_dev.data_ptr(), nnz,
+                                             dev_map.data_ptr(), st)
+  L.check(rc)
   out = (qnums, sdims, dev_map, offs)
   _MAP_CACHE[key] = out
   return out
@@ -412,10 +577,10 @@ def tensordot(a, b, axes):
   mod = a.indices[0].modulus if a.indices else None
   # B's row charge equals A's row charge within a sector (opposite flows on contracted legs);
   sect = []
-  posb = {int(q): i for i, q in enumerate(qb)}
-  posc = {int(q): i for i, q in enumerate(qc)}
+  posb = {_qkey(q): i for i, q in enumerate(qb)}
+  posc = {_qkey(q): i for i, q in enumerate(qc)}
   for i, q in enumerate(qa):
-    q = int(q)
+    q = _qkey(q)
     if q in posb and q in posc:
       j, k = posb[q], posc[q]
       m_, k_ = int(da[i, 0]), int(da[i, 1])
@@ -528,7 +693,8 @@ def _factor_tensors(tensor, nl, qn, ms, ns, kept, l_buf, l_off, r_buf, r_off):
   row-major at l_off[q] / r_off[q] of the packed buffers, keeping the first kept[q] columns of L_q and rows of R_q.
 
   Returns (L, R): L legs = left legs + [bond], bond flow True; R legs = [bond] + right legs, bond flow False
-  (block_sparse/linalg.py:343-392).  The bond carries the sector charge kept[q] times, sector-major."""
+  (block_sparse/linalg.py:343-392).  The bond carries the sector charge kept[q] times, sector-major: (k,) charges for one
+  symmetry, (k, nsym) with the tensor's per-component moduli for a product."""
   be, code = tensor.backend, tensor.data.code
   l_idx, r_idx, bond_q = [], [], []
   for q, k in enumerate(kept):
@@ -538,11 +704,11 @@ def _factor_tensors(tensor, nl, qn, ms, ns, kept, l_buf, l_off, r_buf, r_off):
     b = np.arange(k)
     l_idx.append((l_off[q] + np.arange(m_)[None, :] * r_ + b[:, None]).ravel())      # (k x m): l_q[:, :k].T
     r_idx.append((r_off[q] + b[:, None] * n_ + np.arange(n_)[None, :]).ravel())      # (k x n): r_q[:k, :]
-    bond_q.append(np.full(k, qn[q], dtype=np.int64))
+    bond_q.append(np.repeat(qn[q:q + 1], k, axis=0).astype(np.int64))
   l_data = _take(be, l_buf, _cat(l_idx), code)
   r_data = _take(be, r_buf, _cat(r_idx), code)
   mod = tensor.indices[0].modulus if tensor.indices else None
-  bond_charges = _cat(bond_q)
+  bond_charges = np.concatenate(bond_q) if bond_q else np.zeros((0,) + qn.shape[1:], dtype=np.int64)
   left = [tensor.indices[tensor.order[i]] for i in range(nl)]
   right = [tensor.indices[tensor.order[i]] for i in range(nl, tensor.ndim)]
   bond_l = Index(bond_charges, True, mod)
@@ -602,7 +768,8 @@ def svd(tensor, pivot_axis, max_singular_values=None, max_truncation_error=None,
   s_vals = _take(be, s_buf, _cat([s_off[q] + np.arange(k) for q, k in enumerate(kept) if k]), T.real_code(code))
   ktot = int(np.sum(kept)) if kept else 0
   s_disc = np.concatenate(discarded) if discarded else np.zeros(0)
-  disc_q = _cat([np.full(len(d), qn[q], dtype=np.int64) for q, d in enumerate(discarded)]) if discarded else np.zeros(0, dtype=np.int64)
+  disc_q = [np.repeat(qn[q:q + 1], len(d), axis=0).astype(np.int64) for q, d in enumerate(discarded)]
+  disc_q = np.concatenate(disc_q) if disc_q else np.zeros((0,) + qn.shape[1:], dtype=np.int64)
   return U, dict(values=s_vals, index=U.indices[0], kept=kept, ktot=ktot, discarded=s_disc, discarded_charges=disc_q), V, s_disc
 
 

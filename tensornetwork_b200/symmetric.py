@@ -13,10 +13,12 @@ leg fusion (`reshape`), lazy transposition and every elementwise helper on the n
 host code, inherited unchanged; `tensordot`, `svd`, `qr` and `rq` — where the reference spends its time (SURVEY 8a
 rows a11, a12; `qr` / `rq` at every site of MPS canonicalisation and one-site DMRG) — upload the nnz vectors, run on
 the device and download the result.  `qr` / `rq` build their own sector maps, so they also factor the dimension-1
-boundary legs of a finite MPS, on which the reference's host path fails under numpy 2.  Supported symmetry: ONE
-U(1) / Z_N charge per leg (the reference's product charges raise NotImplementedError here, as do the two
-degenerate forms of tensordot that are not sector contractions: outer product and full inner product go to
-the reference implementation, which is a numpy dot / outer of the data vectors).
+boundary legs of a finite MPS, on which the reference's host path fails under numpy 2.  Supported symmetries: U(1) and
+Z_N charges, and the reference's product charges built from them (a `BaseCharge` with several `charge_types`, e.g.
+U(1) x U(1) for particle number and S_z, or U(1) x Z_2); sectors and bond charges come out in the reference's order.
+Other charge types raise NotImplementedError.  The two degenerate forms of tensordot that are not sector contractions
+(outer product and full inner product) go to the reference implementation, which is a numpy dot / outer of the data
+vectors.
 """
 import numpy as np
 
@@ -27,25 +29,33 @@ _CLASS = None
 
 
 def _modulus(charge):
-  """None for U(1), N for Z_N; raises for anything this adapter does not cover.  The reference builds Z_N classes in a factory
-  (`charge.py:549-600`, class name `ModularCharge`) without recording N; the dual of charge 1 reveals it: -1 for U(1), N-1 for Z_N
-  (Z2: 1)."""
-  types = charge.charge_types
-  if len(types) != 1:
-    raise NotImplementedError("symmetric_b200 supports one symmetry per leg, got a product of {}".format(len(types)))
-  d = int(np.asarray(types[0].dual_charges(np.array([1], dtype=np.int16))).ravel()[0])
-  if d == -1:
-    return None
-  if d >= 1:
-    return d + 1
-  raise NotImplementedError("symmetric_b200: unsupported charge type {}".format(types[0]))
+  """One entry per charge component: None for U(1), N for Z_N; raises for anything this adapter does not cover.  The
+  reference builds Z_N classes in a factory (`charge.py:549-600`, class name `ModularCharge`) without recording N; the dual
+  of charge 1 reveals it: -1 for U(1), N-1 for Z_N (Z2: 1)."""
+  mods = []
+  for t in charge.charge_types:
+    d = int(np.asarray(t.dual_charges(np.array([1], dtype=np.int16))).ravel()[0])
+    if d == -1:
+      mods.append(None)
+    elif d >= 1:
+      mods.append(d + 1)
+    else:
+      raise NotImplementedError("symmetric_b200: unsupported charge type {}".format(t))
+  return tuple(mods)
+
+
+def _bond_charge(tensor, q):
+  """the reference charge object of a bond with charges q ((k,) or (k, nsym)), of the type and charge_types of the
+  tensor's first leg"""
+  c0 = tensor._charges[0]  # pylint: disable=protected-access
+  return type(c0)(np.asarray(q, dtype=np.int16), charge_types=c0.charge_types)
 
 
 def _to_device(tensor, be):
   """reference BlockSparseTensor -> (ours over the ELEMENTARY legs, leg groups): groups[n] = positions (in our logical
   order = the reference's flat order) of the elementary legs of logical leg n."""
   charges, flows = tensor._charges, tensor._flows  # pylint: disable=protected-access
-  indices = [bsp.Index(np.asarray(c.charges)[:, 0].astype(np.int64), bool(f), _modulus(c)) for c, f in zip(charges, flows)]
+  indices = [bsp.Index(np.asarray(c.charges).astype(np.int64), bool(f), _modulus(c)) for c, f in zip(charges, flows)]
   flat, groups, s = [], [], 0
   for leg in tensor._order:  # pylint: disable=protected-access
     flat.extend(int(o) for o in leg)
@@ -118,9 +128,7 @@ def _make_class():
       nl_logical = len(left_dims)
       nl = sum(len(g) for g in groups[:nl_logical])
       U, S, V, _ = bsp.svd(dt, nl, max_singular_values, max_truncation_error, relative)
-      cls = type(tensor._charges[0])  # pylint: disable=protected-access
-      mk = lambda q: cls(np.asarray(q, dtype=np.int16))
-      bond = mk(S["index"].charges)
+      bond = _bond_charge(tensor, S["index"].charges)
       flat = dt.order
       left_c = [tensor._charges[o] for o in flat[:nl]]  # pylint: disable=protected-access
       left_f = [tensor._flows[o] for o in flat[:nl]]  # pylint: disable=protected-access
@@ -131,7 +139,7 @@ def _make_class():
       v = BlockSparseTensor(V.data.to_host(), charges=[bond] + right_c, flows=[False] + right_f,
                             order=[[0], list(range(1, len(right_c) + 1))], check_consistency=False)
       s = ChargeArray(S["values"].to_host(), [bond], [False])
-      sdisc = ChargeArray(S["discarded"], [mk(S["discarded_charges"])], [False])
+      sdisc = ChargeArray(S["discarded"], [_bond_charge(tensor, S["discarded_charges"])], [False])
       k = s.shape[0]
       return u.reshape(tuple(left_dims) + (k,)), s, v.reshape((k,) + tuple(right_dims)), sdisc
 
@@ -143,7 +151,7 @@ def _make_class():
       dt, groups = _to_device(tensor, self.device_backend)
       nl = sum(len(g) for g in groups[:len(left_dims)])
       lf, rf = factor(dt, nl)
-      bond = type(tensor._charges[0])(np.asarray(lf.indices[0].charges, dtype=np.int16))  # pylint: disable=protected-access
+      bond = _bond_charge(tensor, lf.indices[0].charges)
       flat = dt.order
       cf = lambda legs: ([tensor._charges[o] for o in legs], [tensor._flows[o] for o in legs])  # pylint: disable=protected-access
       (left_c, left_f), (right_c, right_f) = cf(flat[:nl]), cf(flat[nl:])
