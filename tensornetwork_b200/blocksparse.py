@@ -617,6 +617,54 @@ def tensordot(a, b, axes):
   return out
 
 
+def _balanced_split(dims):
+  """the k in [1, len(dims)] for which the dense sizes of dims[:k] and dims[k:] are closest"""
+  total, best, split, left = math.prod(dims), None, 1, 1
+  for i in range(1, len(dims) + 1):
+    left *= dims[i - 1]
+    cost = max(left, total // max(left, 1))
+    if best is None or cost < best:
+      best, split = cost, i
+  return split
+
+
+def permutation_map(be, indices, permutation):
+  """Device int64 map of block-sparse transposition (blocksparsetensor.py:803-860 `contiguous`): for a data vector stored
+  over the legs `indices`, data[map] is the data vector stored over the legs [indices[p] for p in permutation], element
+  for element what the reference's `contiguous(permutation)` computes.
+
+  Built once per (legs, permutation) and cached.  Two `_device_sector_maps` with the same row legs list the same elements
+  in the same order (sector after sector, row-major): the source legs viewed in the target order (map_s: positions in the
+  source vector) and the permuted legs in identity order (map_t: positions in the target vector).  So the map is one
+  int64 scatter, map[map_t] = map_s."""
+  permutation = [int(p) for p in permutation]
+  key = ("perm", tuple(ix.key() for ix in indices), tuple(permutation))
+  hit = _MAP_CACHE.get(key)
+  if hit is not None:
+    return hit
+  target = [indices[p] for p in permutation]
+  part = _balanced_split([ix.dim for ix in target])
+  qs, ds, map_s, _ = _device_sector_maps(be, indices, permutation, part)
+  qt, dt, map_t, _ = _device_sector_maps(be, target, list(range(len(target))), part)
+  if not (np.array_equal(qs, qt) and np.array_equal(ds, dt)):
+    raise RuntimeError("block-sparse transposition: sector bookkeeping mismatch (internal error)")
+  nnz = BlockSparseTensor._nnz(indices)  # pylint: disable=protected-access
+  out = be.torch.empty(max(nnz, 1), dtype=be.torch.int64, device=be.device)
+  L.check(be.lib.tnb200_gather(map_s.data_ptr(), map_t.data_ptr(), out.data_ptr(), nnz, L.I64, 1,
+                               be._stream()))  # pylint: disable=protected-access
+  _MAP_CACHE[key] = out
+  return out
+
+
+def gather(be, data, dev_map, n):
+  """data[dev_map[:n]] as a new 1-D device vector (one `tnb200_gather`)."""
+  out = be._new((n,), data.code)  # pylint: disable=protected-access
+  if n:
+    L.check(be.lib.tnb200_gather(data.t.data_ptr(), dev_map.data_ptr(), out.t.data_ptr(), n, data.code, 0,
+                                 be._stream()))  # pylint: disable=protected-access
+  return out
+
+
 # ===================================================================================== svd
 def _truncate_sectors(singvals, max_singular_values=None, max_truncation_error=None, relative=False):
   """The cross-sector truncation of backends/symmetric/decompositions.py:63-136, restated on host
